@@ -12,6 +12,7 @@ weights (no checkpoints offline), fp16 storage + fp32 accumulation like the refe
     python bench.py --impl torch-cuda ...                    the same algorithm through stock PyTorch CUDA ops on this GPU
     python bench.py --views 4 | --res 1024 --dtype bf16 | --views 64 (8 GPUs) | --shading splitsum    BASELINE configs 2 / 3 / 4 / a5
     python bench.py --gpus 2 --check                         + gradient identity of the sharded step vs one process
+    python bench.py --dump-outputs DIR                       + what the last timed step computed, as DIR/<name>.npy
 """
 import argparse
 import json
@@ -28,20 +29,19 @@ UNET_CN_TFLOP_PER_VIEW = 3.27
 
 
 def burst_tflops():
-    """burst bf16/fp16 tensor peak for a kernel timed alone (MEASURED_PEAKS.json `bf16_tflops`), else the recipe's fallback"""
+    """burst bf16/fp16 tensor peak for a kernel timed alone (MEASURED_PEAKS.json `bf16_tflops`), else the H100 SXM data sheet's dense figure"""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f)["bf16_tflops"], "measured"
     except Exception:
-        return 1650.0, "fallback"
+        return 989.0, "H100 SXM data sheet"
 
 
 def kernel_roofline(dtype):
-    """Roofline of the dominant tensor kernel, timed ALONE with CUDA events on the launching stream: the CTA-pair
-    implicit-GEMM convolution on the UNet's 16x16-latent layer of the 8-view batch (conv3x3 24x16x16, 1280 -> 1280).
-    Algorithmic flops per launch = 2 * 6144 * 1280 * 11520; `traffic` is the DRAM read+write of the same launch from the
-    committed ncu --set full capture (profiles/r01c_launches_summary.md: 45.3 + 1.3 MB; algorithmic 29.5 MB weights +
-    15.7 MB input + 15.7 MB output, the nine taps re-read L2 only)."""
+    """Roofline of the dominant tensor kernel, timed ALONE with CUDA events on the launching stream: the implicit-GEMM
+    convolution on the UNet's 16x16-latent layer of the 8-view batch (conv3x3 24x16x16, 1280 -> 1280).
+    Algorithmic flops per launch = 2 * 6144 * 1280 * 11520; `traffic` is the algorithmic DRAM bytes of the launch
+    (29.5 MB weights + 15.7 MB input + 15.7 MB output; the nine taps re-read L2 only)."""
     import torch
     from dreammat_b200 import dense_ops as D
     x = torch.randn(24, 16, 16, 1280, device="cuda").to(dtype)
@@ -60,9 +60,9 @@ def kernel_roofline(dtype):
     flops = 2.0 * 24 * 256 * 1280 * 1280 * 9
     peak, src = burst_tflops()
     ach = flops / (ms * 1e-3) / 1e12
-    return {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": 46.6e6,
-            "kernel": "tc_gemm_pair_kernel<256> conv3x3 24x16x16 1280->1280 (timed alone, %d launches, %.1f us each)" % (n, ms * 1e3),
-            "peak_source": src + " burst bf16", "traffic_source": "ncu --set full, profiles/r01c_launches_summary.md"}
+    return {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": 60.9e6,
+            "kernel": "tc_gemm_kernel conv3x3 24x16x16 1280->1280 (timed alone, %d launches, %.1f us each)" % (n, ms * 1e3),
+            "peak_source": src + " burst bf16", "traffic_source": "algorithmic bytes"}
 
 
 def peaks():
@@ -71,7 +71,7 @@ def peaks():
             p = json.load(f)
         return p["hbm_gbs"], p.get("bf16_tflops_sustained", p["bf16_tflops"]), "measured"
     except Exception:
-        return 6650.0, 1400.0, "fallback"
+        return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -151,9 +151,6 @@ def build_system(device, res, n_faces, env_hw, seed, dtype, shading="mc"):
     return sysm, cams
 
 
-FP32_LANES_PER_SM = 128
-
-
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -166,7 +163,8 @@ def run_ours(args):
         # NCCL_DEBUG is left exactly as the launcher set it (its banner goes to stderr with everything else, see main())
         dist.init_process_group("nccl", device_id=torch.device(device))
     from dreammat_b200 import _cabi
-    _cabi.check(_cabi.lib().dm_device_check(local), "dm_device_check")   # fails loudly without the sm_100a library
+    _cabi.check(_cabi.lib().dm_device_check(local), "dm_device_check")   # fails loudly without the sm_90a library
+    torch.manual_seed(0)       # the step's device-side draws (MC directions, jitter, timesteps, noise) repeat run to run
     if args.no_pdl:
         _cabi.lib().dm_tune(b"pdl", 0)
     dtype = torch.bfloat16 if args.dtype == "bf16" else torch.float16
@@ -233,12 +231,14 @@ def run_ours(args):
             return None
 
     h2d_seen = {}
+    last = {}
 
     def step(mode="device"):
         b, tot_pn, h2d = make_batch(mode)
         h2d_seen[mode] = h2d
         b["rays_o"] = b["rays_d"] = _Rays()
         out = sysm.training_step_fused(b, global_views=V, total_pn_global=tot_pn)
+        last["out"] = out
         if mode != "device":
             return float(out["loss"])      # D2H read of the step's result
         return out["loss"]
@@ -279,6 +279,8 @@ def run_ours(args):
 
     sampler = ClockSampler(local) if rank == 0 else None
     ms_step, launches, spread = timed(args.warmup, args.steps, "device")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"], sysm.geometry)
     # section split (one extra profiled step, outside the timed region)
     sec = sysm.profile_step(lambda: make_batch("device")[:2], V) if hasattr(sysm, "profile_step") else {}
     ms_e2e, _, spread_e2e = timed(max(1, args.warmup // 2), args.steps, "e2e")
@@ -303,7 +305,7 @@ def run_ours(args):
                           cfg_name, res, res, V, Vl, "200+128 MC rays/px" if args.shading == "mc" else "split-sum shading"),
                       "views": V, "resolution": res, "shading": args.shading,
                       "parallelism": "dp%d (views sharded; shading pixels balanced over ranks by 2 small all-to-alls; 1 all-reduce of 50.4 MB grads)" % world,
-                      "l2": "working set (2.5 GB weights + activations) exceeds the 126 MB L2 every step",
+                      "l2": "working set (2.5 GB weights + activations) exceeds the 50 MB L2 every step",
                       "g_buffer": "rasterisation (row a2) is hoisted out of the step: fixed mesh + 128 fixed cameras -> per-view G-buffer cache built before timing",
                       "condition_maps": "resident on the device as uint8 (%.2f GB), gathered by (view, env) id inside the ControlNet graph" % (maps.nbytes / 1e9)},
            "step_time_spread": spread, "clocks": clocks, "gpu_launches": int(launches),
@@ -317,7 +319,7 @@ def run_ours(args):
     if t_dense:
         ach = DENSE_TFLOP_PER_VIEW * Vl / (t_dense / 1000.0)
         out["roofline"] = {"bound": "tensor", "achieved": ach, "peak": tf, "unit": "TFLOP/s", "frac": ach / tf,
-                           "traffic": None, "kernel": "tc_gemm_pair_kernel + tc_gemm_kernel + attention_kernel over the dense section",
+                           "traffic": None, "kernel": "tc_gemm_kernel + attention_kernel over the dense section",
                            "peak_source": src + " sustained bf16",
                            "note": "section-level: algorithmic flops of ALL dense kernels / CUDA-event time of the section inside the timed "
                                    "step (GroupNorm, softmax etc. included); the dominant tensor kernel alone is in roofline_kernel, the "
@@ -330,19 +332,13 @@ def run_ours(args):
         t_r = sec.get("render_fwd_ms")
         if t_r:
             pn_step = float(sec.get("pn_local", 0))
-            sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-            fp32_peak = 148 * FP32_LANES_PER_SM * 2 * sm_mhz * 1e6
             if args.shading == "mc":
-                # NOT HBM-bound (BVH traversal + FP32 ALU).  SURVEY 8d: rays/s, the FP32-lane fraction and the HBM fraction
-                # from the byte formula (200 B per covered pixel + one 16 B texel per unoccluded sample; upper bound: every sample)
+                # NOT HBM-bound (BVH traversal + FP32 ALU).  SURVEY 8d: rays/s and the HBM fraction from the byte formula
+                # (200 B per covered pixel + one 16 B texel per unoccluded sample; upper bound: every sample)
                 byts = pn_step * (200.0 + 16.0 * 328)
-                instr = MC_THREAD_INSTR_PER_RAY * pn_step * 328
                 out["roofline_shading"] = {"bound": "hbm", "achieved": byts / (t_r * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s",
                                            "frac": byts / (t_r * 1e-3) / 1e9 / hbm, "traffic": None,
                                            "rays_per_s": pn_step * 328 / (t_r * 1e-3), "covered_pixels": pn_step,
-                                           "fp32_frac": 2.0 * instr / (t_r * 1e-3) / fp32_peak,
-                                           "fp32_note": "lane-level instructions of the shader (ncu smsp__thread_inst_executed, %d per ray, "
-                                                        "profiles/r02_shade_frontier.md) x 2 flop / (148 SM x 128 lanes x 2 x %.0f MHz)" % (MC_THREAD_INSTR_PER_RAY, sm_mhz),
                                            "note": "latency/issue-bound BVH any-hit traversal (shared-origin frontier); bytes are an upper bound (every sample unoccluded)"}
             else:
                 byts = pn_step * 124.0          # forward only inside render_fwd (76 B more in the backward section)
@@ -363,7 +359,32 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
-MC_THREAD_INSTR_PER_RAY = 2290     # measured: ncu thread-level instructions of shade_mc_kernel / rays (profiles/r02_shade_frontier.md)
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(d, out, geo, sample=1 << 20, max_pixels=1 << 21):
+    """What the last timed step handed its caller (loss terms, logged norms, the rendered batch) and the state it left
+    (parameters after Adam, their gradient), as float32 .npy files, DUMP_LIMIT bytes at most; the two flat 12.6 M-entry
+    vectors are sampled at the same seeded 1 M indices every run (4 MB each), and a rendered batch of more than 2 M pixels
+    (the default 8 x 512^2 is exactly that) at the same seeded 2 M pixels, so two builds can be compared output for output."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    arrays = {k: v for k, v in out.items() if torch.is_tensor(v)}
+    idx = torch.randperm(geo.params.numel(), generator=torch.Generator().manual_seed(0))[:sample].sort().values
+    arrays["params_sample"] = geo.params.detach().cpu()[idx]
+    arrays["grads_sample"] = geo.grads.detach().cpu()[idx]
+    arrays["sample_index"] = idx.double()
+    rgb = arrays["comp_rgb"].reshape(-1, arrays["comp_rgb"].shape[-1])
+    if rgb.shape[0] > max_pixels:
+        pix = torch.randperm(rgb.shape[0], generator=torch.Generator().manual_seed(1))[:max_pixels].sort().values
+        arrays["comp_rgb"] = rgb[pix.to(rgb.device)]
+        arrays["comp_rgb_pixel_index"] = pix.double()
+    arrays = {k: (v.detach().float().cpu() if v.dtype != torch.float64 else v.cpu()).numpy() for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT, f"output dump of {total} bytes exceeds {DUMP_LIMIT}"
+    for k, a in arrays.items():
+        np.save(os.path.join(d, k + ".npy"), a)
 
 
 def splitsum_kernel_roofline(sysm, hbm):
@@ -461,8 +482,8 @@ def gradient_identity_check(sysm, make_batch, cam_dev, V, world, rank, device):
                 sysm.training_step_fused(full, global_views=V, total_pn_global=tot_pn, rng=rng, apply_optimizer=False)
                 g_single = geo.grads.clone()
                 err = float((g_sharded.double() - g_single.double()).norm() / (g_single.double().norm() + 1e-30))
-                # the same single-process evaluation once more: its own run-to-run noise (fp32 atomics in split-K / GroupNorm
-                # statistics / hash-grid scatter) is the floor the sharded result has to be read against
+                # the same single-process evaluation once more: its run-to-run difference (0: the step is deterministic) is
+                # the floor the sharded result has to be read against
                 restore()
                 sysm.training_step_fused(full, global_views=V, total_pn_global=tot_pn, rng=rng, apply_optimizer=False)
                 floor = float((geo.grads.double() - g_single.double()).norm() / (g_single.double().norm() + 1e-30))
@@ -754,6 +775,7 @@ def main():
     ap.add_argument("--no-pdl", action="store_true", help="disable programmatic dependent launch of the dense kernels")
     ap.add_argument("--no-gc-freeze", action="store_true", help="A/B: leave Python's full collections inside the timed region")
     ap.add_argument("--no-balance", action="store_true", help="multi-GPU: every rank shades only its own views")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (float32/float64, <= 64 MB)")
     args = ap.parse_args()
     # stdout carries exactly one JSON line: libraries that write to fd 1 (NCCL's version banner, nvcc/ninja chatter)
     # are sent to stderr for the whole run and the result line is written to the saved descriptor.

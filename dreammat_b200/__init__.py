@@ -1,4 +1,4 @@
-"""dreammat_b200 -- B200-native (sm_100a) score-distillation inner loop for DreamMat.
+"""dreammat_b200 -- H100-native (sm_90a) score-distillation inner loop for DreamMat.
 
 The package holds only what the hot path needs: `csrc/` (CUDA kernels + the C-ABI of
 include/dreammat_b200.h), thin torch-facing wrappers, and host-side mirrors of the five

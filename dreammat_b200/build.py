@@ -1,4 +1,4 @@
-"""Build libdreammat_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libdreammat_b200.so (sm_90a only) in-tree with nvcc.
 
 The shared object is the product's C-ABI (include/dreammat_b200.h); it lives next to the
 package so it travels with the repo snapshot to the GPU box.
@@ -14,7 +14,7 @@ LIB = os.path.join(LIBDIR, "libdreammat_b200.so")
 OBJDIR = os.path.join(HERE, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -51,7 +51,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if failed:
         raise RuntimeError("nvcc build failed")
     if procs or force or not os.path.exists(LIB):
-        cmd = ["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = ["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         subprocess.check_call(cmd)
     return LIB
 

@@ -1,4 +1,4 @@
-// attention.cu -- fused softmax(Q K^T / sqrt(d)) V for head_dim 64 on tcgen05 tensor cores.
+// attention.cu -- fused softmax(Q K^T / sqrt(d)) V for head_dim 64 on Hopper wgmma tensor cores.
 //
 // Replaces torch SDPA / diffusers AttnProcessor inside BasicTransformerBlock (self-attention,
 // N = 4096 / 1024 / 256 / 64 tokens, and cross-attention over the 77 text tokens) for the UNet and
@@ -9,16 +9,11 @@
 // head slice; no split-heads copies.  O is written back in the same layout.
 //
 // One CTA = 128 queries of one (batch, head); keys are streamed in blocks of 64:
-//   warp 0   TMA producer: Q once, then a ring of K/V stages
-//   warp 1   MMA issuer:   S = Q K_j^T  (M128 N64 K64, accumulator in TMEM)
-//                          O_j = P_j V_j (A = P_j from shared memory, B = V_j as an MN-major operand)
-//   warps 2-5 softmax:     thread r owns query row r: tcgen05.ld of its S row, online max / exp2 / sum,
-//                          P_j -> fp16 into the 128B-swizzled K-major tile, O accumulated in registers
-//                          (O_j is read back from TMEM one block late, so the tensor pipe never waits
-//                          for the rescale).
-// Two CTAs are resident per SM (<= 96 KB smem, 256 TMEM columns each; S is double-buffered in TMEM): while one CTA's softmax
-// warps work through their exponentials (the MUFU unit, not the tensor pipe, bounds head_dim 64
-// attention), the other CTA's MMAs run.
+//   warp 8      TMA producer: Q once, then a ring of K/V stages
+//   warps 0-7   two consumer warpgroups, 64 query rows each:
+//               S = Q K_j^T   (m64n64k16, both operands in shared memory, accumulator in registers)
+//               online max / exp2 / sum on the S fragment (a row lives in the 4 lanes of a quad)
+//               O += P_j V_j  (P_j straight from registers as the A operand, V_j an MN-major shared-memory operand)
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -31,12 +26,10 @@ constexpr int AQ = 128;       // queries per CTA
 constexpr int AK = 64;        // keys per block
 constexpr int HD = 64;        // head dim
 constexpr int KV_STAGES = 3;
-constexpr int ATT_THREADS = 192;
+constexpr int ATT_THREADS = 288;
 constexpr int Q_BYTES = AQ * HD * 2;     // 16 KB
 constexpr int KV_BYTES = AK * HD * 2;    // 8 KB
-constexpr int P_BYTES = AQ * AK * 2;     // 16 KB
-constexpr int ATT_SMEM = Q_BYTES + 2 * KV_STAGES * KV_BYTES + P_BYTES + 1024 + 256;
-constexpr int ATT_TMEM_COLS = 256;       // S double buffer: cols [0,64) and [64,128); O_j: cols [128,192)
+constexpr int ATT_SMEM = Q_BYTES + 2 * KV_STAGES * KV_BYTES + 1024 + 256;
 
 struct AttnParams {
     int Nq, Nk, heads;
@@ -44,18 +37,11 @@ struct AttnParams {
     float scale_log2e;   // (1/sqrt(d)) * log2(e)
 };
 
-// MN-major 128B-swizzled operand (V: rows = keys (K dim), 64 contiguous head-dim elements per row)
-__device__ __forceinline__ uint64_t make_sw128_desc_mn(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (64ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
 __device__ __forceinline__ float fast_exp2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-
-int g_attn_packed_exp = 0;   // dm_tune_attention(1): packed f16x2 exponentials (experiment)
 
 template <typename T> struct PK;
 template <> struct PK<__half> {
@@ -63,83 +49,35 @@ template <> struct PK<__half> {
         __half2 h = __floats2half2_rn(a, b);
         return *reinterpret_cast<uint32_t*>(&h);
     }
-    // P row block = exp2(s*scale - max) for 64 keys, packed for the PV MMA, plus its row sum.
-    // The softmax warps are bound by the MUFU pipe (one ex2 per score: 4.5 T/s chip-wide, ncu profiles/r01b), so the
-    // fp16 path evaluates TWO exponentials per MUFU op (ex2.approx.f16x2 on the packed, already max-subtracted
-    // argument) -- the result is directly the fp16 pair the tensor core consumes.  The row sum is formed from those
-    // rounded values (two packed-add levels, then fp32), i.e. it normalises exactly what the MMA multiplies.
-    template <bool PACKED>
-    static __device__ __forceinline__ float exp_block(const uint32_t (&sv)[64], float scale, float neg_mx, uint32_t (&pk)[32]) {
-        if (!PACKED) {
-            float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;      // independent partial row sums (no 64-long FADD chain)
-#pragma unroll
-            for (int c = 0; c < 64; c += 4) {
-                float p0 = fast_exp2(fmaf(__uint_as_float(sv[c]), scale, neg_mx));
-                float p1 = fast_exp2(fmaf(__uint_as_float(sv[c + 1]), scale, neg_mx));
-                float p2 = fast_exp2(fmaf(__uint_as_float(sv[c + 2]), scale, neg_mx));
-                float p3 = fast_exp2(fmaf(__uint_as_float(sv[c + 3]), scale, neg_mx));
-                l0 += p0; l1 += p1; l2 += p2; l3 += p3;
-                pk[c >> 1] = pack(p0, p1);
-                pk[(c >> 1) + 1] = pack(p2, p3);
-            }
-            return (l0 + l1) + (l2 + l3);
-        }
-#pragma unroll
-        for (int c = 0; c < 64; c += 2) {
-            __half2 x = __floats2half2_rn(fmaf(__uint_as_float(sv[c]), scale, neg_mx), fmaf(__uint_as_float(sv[c + 1]), scale, neg_mx));
-            uint32_t xi = *reinterpret_cast<uint32_t*>(&x), yi;
-            asm("ex2.approx.f16x2 %0, %1;" : "=r"(yi) : "r"(xi));
-            pk[c >> 1] = yi;
-        }
-        float lsum = 0.f;
-#pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-            __half2 a = __hadd2(*reinterpret_cast<const __half2*>(&pk[c]), *reinterpret_cast<const __half2*>(&pk[c + 1]));
-            __half2 b = __hadd2(*reinterpret_cast<const __half2*>(&pk[c + 2]), *reinterpret_cast<const __half2*>(&pk[c + 3]));
-            float2 f = __half22float2(__hadd2(a, b));
-            lsum += f.x + f.y;
-        }
-        return lsum;
-    }
 };
 template <> struct PK<__nv_bfloat16> {
     static __device__ __forceinline__ uint32_t pack(float a, float b) {
         __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
         return *reinterpret_cast<uint32_t*>(&h);
     }
-    // bf16 keeps the fp32 exponentials (8 mantissa bits are too few for packed sums)
-    template <bool PACKED>
-    static __device__ __forceinline__ float exp_block(const uint32_t (&sv)[64], float scale, float neg_mx, uint32_t (&pk)[32]) {
-        float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 64; c += 4) {
-            float p0 = fast_exp2(fmaf(__uint_as_float(sv[c]), scale, neg_mx));
-            float p1 = fast_exp2(fmaf(__uint_as_float(sv[c + 1]), scale, neg_mx));
-            float p2 = fast_exp2(fmaf(__uint_as_float(sv[c + 2]), scale, neg_mx));
-            float p3 = fast_exp2(fmaf(__uint_as_float(sv[c + 3]), scale, neg_mx));
-            l0 += p0; l1 += p1; l2 += p2; l3 += p3;
-            pk[c >> 1] = pack(p0, p1);
-            pk[(c >> 1) + 1] = pack(p2, p3);
-        }
-        return (l0 + l1) + (l2 + l3);
-    }
 };
 
-template <typename T, int MODE>   // MODE 0: fp32 exponentials, rescale every block; 1: packed f16x2 exp + lazy rescale; 2: fp32 exp + lazy rescale
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+template <typename T>
 __global__ void __launch_bounds__(ATT_THREADS, 2) attention_kernel(const __grid_constant__ CUtensorMap tmQ,
                                                                    const __grid_constant__ CUtensorMap tmK,
                                                                    const __grid_constant__ CUtensorMap tmV,
                                                                    const AttnParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t sQ = base, sK = sQ + Q_BYTES, sV = sK + KV_STAGES * KV_BYTES, sP = sV + KV_STAGES * KV_BYTES;
-    const uint32_t bars = sP + P_BYTES;
+    const uint32_t sQ = base, sK = sQ + Q_BYTES, sV = sK + KV_STAGES * KV_BYTES;
+    const uint32_t bars = sV + KV_STAGES * KV_BYTES;
     const uint32_t q_full = bars;
     auto kv_full = [&](int s) { return bars + 8u * (1 + s); };
     auto kv_empty = [&](int s) { return bars + 8u * (1 + KV_STAGES + s); };
-    const uint32_t s_full0 = bars + 8u * (1 + 2 * KV_STAGES), p_full = s_full0 + 16u, o_full = p_full + 8u;
-    auto s_full = [&](int jj) { return s_full0 + 8u * (uint32_t)(jj & 1); };
-    const uint32_t tmem_slot = o_full + 8u;
 
     griddep_launch_dependents();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -149,20 +87,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attention_kernel(const __grid_
     if (threadIdx.x == 0) {
         prefetch_tmap(&tmQ); prefetch_tmap(&tmK); prefetch_tmap(&tmV);
         mbar_init(q_full, 1);
-        for (int s = 0; s < KV_STAGES; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); }
-        mbar_init(s_full(0), 1); mbar_init(s_full(1), 1); mbar_init(p_full, 128); mbar_init(o_full, 1);
+        for (int s = 0; s < KV_STAGES; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 2); }
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, ATT_TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = ld_shared_u32(tmem_slot);
     griddep_wait();      // PDL: q/k/v written by the previous kernel are visible from here
-    const uint32_t tmem_O = tmem + 128;
-    auto tmem_S = [&](int jj) { return tmem + 64u * (uint32_t)(jj & 1); };
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             mbar_expect_tx(q_full, Q_BYTES);
             tma_load_3d(sQ, &tmQ, q_full, head * HD, q_tile * AQ, b);
@@ -175,162 +106,88 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attention_kernel(const __grid_
                 if (++stage == KV_STAGES) { stage = 0; phase ^= 1u; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t FMT = std::is_same<T, __half>::value ? 0u : 1u;
-            // S: A = Q (K-major), B = K (K-major), M=128, N=64
-            constexpr uint32_t IDESC_S = (1u << 4) | (FMT << 7) | (FMT << 10) | ((uint32_t)(AK >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-            // O: A = P (K-major), B = V (MN-major: bit 16), M=128, N=64
-            constexpr uint32_t IDESC_O = (1u << 4) | (FMT << 7) | (FMT << 10) | (1u << 16) | ((uint32_t)(HD >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-            const uint64_t dQ = make_sw128_desc(sQ), dP = make_sw128_desc(sP);
-            mbar_wait(q_full, 0);
-            int stage = 0; uint32_t phase = 0;       // stage / phase of block j (V_j, and K_j already consumed)
-            int kstage = 0; uint32_t kphase = 0;     // stage / phase of the next K block to turn into S
-            // S(0)
-            mbar_wait(kv_full(0), 0);
-            tc_fence_after();
-#pragma unroll
-            for (int k = 0; k < HD / 16; ++k) umma_f16(tmem_S(0), dQ + 2 * k, make_sw128_desc(sK) + 2 * k, IDESC_S, k != 0);
-            umma_commit(s_full(0));
-            if (++kstage == KV_STAGES) { kstage = 0; kphase ^= 1u; }
-            for (int j = 0; j < nkb; ++j) {
-                // S(j+1) goes into the other S buffer right away, so the softmax warps never wait for the tensor pipe.
-                // That buffer held S(j-1), which the softmax warps finished reading before they published P(j-1).
-                if (j + 1 < nkb) {
-                    mbar_wait(kv_full(kstage), kphase);
-                    tc_fence_after();
-                    const uint64_t dK = make_sw128_desc(sK + kstage * KV_BYTES);
-#pragma unroll
-                    for (int k = 0; k < HD / 16; ++k) umma_f16(tmem_S(j + 1), dQ + 2 * k, dK + 2 * k, IDESC_S, k != 0);
-                    umma_commit(s_full(j + 1));
-                    if (++kstage == KV_STAGES) { kstage = 0; kphase ^= 1u; }
-                }
-                // O_j = P_j V_j once the softmax warps have published P_j
-                mbar_wait(p_full, (uint32_t)(j & 1));
-                tc_fence_after();
-                const uint64_t dV = make_sw128_desc_mn(sV + stage * KV_BYTES);
-#pragma unroll
-                for (int k = 0; k < AK / 16; ++k) umma_f16(tmem_O, dP + 2 * k, dV + (uint64_t)(128 * k), IDESC_O, k != 0);
-                umma_commit(o_full);
-                umma_commit(kv_empty(stage));
-                if (++stage == KV_STAGES) { stage = 0; phase ^= 1u; }
-            }
-        }
-    } else {
-        const int quarter = warp & 3;
-        const int row = quarter * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-        float acc[HD];
-#pragma unroll
-        for (int c = 0; c < HD; ++c) acc[c] = 0.f;
-        float m_run = -INFINITY, l_run = 0.f;
-        const uint32_t p_row = sP + (uint32_t)row * 128u;
-        for (int j = 0; j < nkb; ++j) {
-            mbar_wait(s_full(j), (uint32_t)((j >> 1) & 1));
-            tc_fence_after();
-            uint32_t sv[64];
-            {
-                uint32_t t0[32], t1[32];
-                tmem_ld_32x32b_x32(tmem_S(j) + lane_addr, t0);
-                tmem_ld_32x32b_x32(tmem_S(j) + lane_addr + 32, t1);
-                tmem_ld_wait();
-#pragma unroll
-                for (int c = 0; c < 32; ++c) { sv[c] = t0[c]; sv[32 + c] = t1[c]; }
-            }
-            const int kvalid = p.Nk - j * AK;  // keys of this block that exist
-            float mraw = -INFINITY;
-            if (kvalid >= AK) {
-                // four independent running maxima: a single 64-long dependent FMNMX chain costs ~250 cycles of latency per block
-                float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-                for (int c = 0; c < AK; c += 4) {
-                    m0 = fmaxf(m0, __uint_as_float(sv[c])); m1 = fmaxf(m1, __uint_as_float(sv[c + 1]));
-                    m2 = fmaxf(m2, __uint_as_float(sv[c + 2])); m3 = fmaxf(m3, __uint_as_float(sv[c + 3]));
-                }
-                mraw = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-            } else {            // ragged last block (cross-attention over 77 tokens): mask the missing keys
-#pragma unroll
-                for (int c = 0; c < AK; ++c) {
-                    float s = (c < kvalid) ? __uint_as_float(sv[c]) : -INFINITY;
-                    sv[c] = __float_as_uint(s);
-                    mraw = fmaxf(mraw, s);
-                }
-            }
-            // Lazy rescaling: the reference max only moves when some row's new maximum exceeds it by more than 2^8 (P then
-            // stays <= 256, exact in fp16/fp32); otherwise alpha == 1 and the 64-register rescale is skipped.  The final
-            // O / l division cancels the stale reference exactly.
-            const float mx_new = fmaxf(m_run, mraw * p.scale_log2e);   // running max in the scaled (log2) domain
-            constexpr bool PACKED = (MODE == 1);
-            constexpr bool LAZY = (MODE != 0);
-            const bool need = !LAZY || !(mx_new - m_run <= 8.0f);     // also true on the first block (m_run = -inf)
-            const bool any_need = !LAZY || __any_sync(0xffffffffu, need);
-            const float mx = need ? mx_new : m_run;
-            uint32_t pk[32];
-            const float lsum = PK<T>::template exp_block<PACKED>(sv, p.scale_log2e, -mx, pk);
-            // previous block's O_j (computed against the previous max) joins the accumulator before the rescale
-            if (j > 0) {
-                mbar_wait(o_full, (uint32_t)((j - 1) & 1));
-                tc_fence_after();
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    uint32_t t0[32];
-                    tmem_ld_32x32b_x32(tmem_O + lane_addr + 32 * hh, t0);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int c = 0; c < 32; ++c) acc[32 * hh + c] += __uint_as_float(t0[c]);
-                }
-            }
-            if (any_need) {
-                const float alpha = fast_exp2(m_run - mx);             // m_run = -inf on the first block -> 0
-#pragma unroll
-                for (int c = 0; c < HD; ++c) acc[c] *= alpha;
-                l_run = l_run * alpha + lsum;
-                m_run = mx;
-            } else {
-                l_run += lsum;
-            }
-            // P_j -> shared memory, 128B-swizzled K-major tile (16-byte chunk index XOR row%8)
-#pragma unroll
-            for (int ch = 0; ch < 8; ++ch) {
-                uint32_t addr = p_row + (uint32_t)((ch ^ (row & 7)) << 4);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pk[4 * ch]), "r"(pk[4 * ch + 1]),
-                             "r"(pk[4 * ch + 2]), "r"(pk[4 * ch + 3]) : "memory");
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            tc_fence_before();
-            mbar_arrive(p_full);
-        }
-        // last block's O
-        mbar_wait(o_full, (uint32_t)((nkb - 1) & 1));
-        tc_fence_after();
-        {
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                uint32_t t0[32];
-                tmem_ld_32x32b_x32(tmem_O + lane_addr + 32 * hh, t0);
-                tmem_ld_wait();
-#pragma unroll
-                for (int c = 0; c < 32; ++c) acc[32 * hh + c] += __uint_as_float(t0[c]);
-            }
-        }
-        const int q = q_tile * AQ + row;
-        if (q < p.Nq) {
-            const float inv = 1.0f / l_run;
-            T* o = reinterpret_cast<T*>(p.out) + (int64_t)b * p.out_batch_stride + (int64_t)q * p.ldo + head * HD;
-#pragma unroll
-            for (int ch = 0; ch < 8; ++ch) {
-                uint4 u;
-                u.x = PK<T>::pack(acc[8 * ch] * inv, acc[8 * ch + 1] * inv);
-                u.y = PK<T>::pack(acc[8 * ch + 2] * inv, acc[8 * ch + 3] * inv);
-                u.z = PK<T>::pack(acc[8 * ch + 4] * inv, acc[8 * ch + 5] * inv);
-                u.w = PK<T>::pack(acc[8 * ch + 6] * inv, acc[8 * ch + 7] * inv);
-                reinterpret_cast<uint4*>(o)[ch] = u;
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, ATT_TMEM_COLS);
+    const int wg = warp >> 2;
+    const int quad_col = 2 * (lane & 3);                       // fragment columns 8j + quad_col + {0, 1}
+    const uint64_t dQ = make_sw128_desc(sQ + (uint32_t)wg * (64 * 128));
+    float o[HD / 2];
+#pragma unroll
+    for (int c = 0; c < HD / 2; ++c) o[c] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // rows r and r + 8 (log2 domain max, partial sums)
+    mbar_wait(q_full, 0);
+    int stage = 0; uint32_t phase = 0;
+    for (int j = 0; j < nkb; ++j) {
+        mbar_wait(kv_full(stage), phase);
+        float s[AK / 2];
+#pragma unroll
+        for (int c = 0; c < AK / 2; ++c) s[c] = 0.f;
+        const uint64_t dK = make_sw128_desc(sK + stage * KV_BYTES);
+        wgmma_fence();
+        wgmma_fence_operands(s);
+#pragma unroll
+        for (int k = 0; k < HD / 16; ++k) Wgmma<AK, T>::ss(s, dQ + (uint64_t)(2 * k), dK + (uint64_t)(2 * k));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(s);
+        const int kvalid = p.Nk - j * AK;    // keys of this block that exist
+        if (kvalid < AK) {                   // ragged last block (cross-attention over 77 tokens): mask the missing keys
+#pragma unroll
+            for (int c = 0; c < AK / 2; ++c)
+                if (8 * (c >> 2) + quad_col + (c & 1) >= kvalid) s[c] = -INFINITY;
+        }
+        float alpha[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float mx = -INFINITY;
+#pragma unroll
+            for (int jj = 0; jj < AK / 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]));
+            const float m_new = fmaxf(m_run[h], quad_max(mx) * p.scale_log2e);
+            alpha[h] = fast_exp2(m_run[h] - m_new);             // m_run = -inf on the first block -> 0
+            m_run[h] = m_new;
+            float l = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < AK / 8; ++jj) {
+                float* v = &s[4 * jj + 2 * h];
+                v[0] = fast_exp2(fmaf(v[0], p.scale_log2e, -m_new));
+                v[1] = fast_exp2(fmaf(v[1], p.scale_log2e, -m_new));
+                l += v[0] + v[1];
+            }
+            l_run[h] = l_run[h] * alpha[h] + l;
+        }
+#pragma unroll
+        for (int jj = 0; jj < HD / 8; ++jj) {
+            o[4 * jj] *= alpha[0]; o[4 * jj + 1] *= alpha[0];
+            o[4 * jj + 2] *= alpha[1]; o[4 * jj + 3] *= alpha[1];
+        }
+        // the S accumulator fragment of columns [16kk, 16kk+16) is the A-operand fragment of k-step kk
+        const uint64_t dV = make_sw128_desc_mn(sV + stage * KV_BYTES);
+        uint32_t a[AK / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < AK / 16; ++kk)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) a[kk][r] = PK<T>::pack(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+        wgmma_fence();
+        wgmma_fence_operands(o);
+#pragma unroll
+        for (int kk = 0; kk < AK / 16; ++kk) Wgmma<HD, T>::rs_bt(o, a[kk], dV + (uint64_t)(128 * kk));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(o);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty(stage));
+        if (++stage == KV_STAGES) { stage = 0; phase ^= 1u; }
+    }
+    const int row = q_tile * AQ + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int q = row + 8 * h;
+        const float inv = 1.0f / quad_sum(l_run[h]);
+        if (q >= p.Nq) continue;
+        T* orow = reinterpret_cast<T*>(p.out) + (int64_t)b * p.out_batch_stride + (int64_t)q * p.ldo + head * HD;
+#pragma unroll
+        for (int jj = 0; jj < HD / 8; ++jj)
+            *reinterpret_cast<uint32_t*>(orow + 8 * jj + quad_col) = PK<T>::pack(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+    }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -358,7 +215,11 @@ int encode3(CUtensorMap* m, int bf16, const void* base, uint64_t cols, uint64_t 
 
 }  // namespace
 
-extern "C" int dm_tune_attention(int mode) { g_attn_packed_exp = (mode == 1 || mode == 2) ? mode : 0; return DM_OK; }
+extern "C" int dm_tune_attention(int mode) {
+    if (mode == 0) return DM_OK;
+    dm_set_error("dm_tune_attention: mode %d does not exist (0 = fp32 exponentials, rescale every block)", mode);
+    return DM_EINVAL;
+}
 
 extern "C" int dm_attention(int bf16, const void* q, int64_t ldq, int64_t q_batch_stride, const void* k, const void* v,
                             int64_t ldkv, int64_t kv_batch_stride, void* out, int64_t ldo, int64_t out_batch_stride,
@@ -381,18 +242,11 @@ extern "C" int dm_attention(int bf16, const void* q, int64_t ldq, int64_t q_batc
     dim3 grid((unsigned)dm_ceil_div(Nq, AQ), (unsigned)heads, (unsigned)batch);
     static bool cfg_h = false, cfg_b = false;
     if (bf16) {
-        if (!cfg_b) { DM_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<__nv_bfloat16, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM)); cfg_b = true; }
-        DM_CHECK_CUDA(dm_launch(attention_kernel<__nv_bfloat16, 0>, grid, dim3(ATT_THREADS), (size_t)ATT_SMEM, (cudaStream_t)stream, tq, tk, tv, p));
+        if (!cfg_b) { DM_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM)); cfg_b = true; }
+        DM_CHECK_CUDA(dm_launch(attention_kernel<__nv_bfloat16>, grid, dim3(ATT_THREADS), (size_t)ATT_SMEM, (cudaStream_t)stream, tq, tk, tv, p));
     } else {
-        if (!cfg_h) {
-            DM_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<__half, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-            DM_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<__half, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-            DM_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<__half, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-            cfg_h = true;
-        }
-        if (g_attn_packed_exp == 1) DM_CHECK_CUDA(dm_launch(attention_kernel<__half, 1>, grid, dim3(ATT_THREADS), (size_t)ATT_SMEM, (cudaStream_t)stream, tq, tk, tv, p));
-        else if (g_attn_packed_exp == 2) DM_CHECK_CUDA(dm_launch(attention_kernel<__half, 2>, grid, dim3(ATT_THREADS), (size_t)ATT_SMEM, (cudaStream_t)stream, tq, tk, tv, p));
-        else DM_CHECK_CUDA(dm_launch(attention_kernel<__half, 0>, grid, dim3(ATT_THREADS), (size_t)ATT_SMEM, (cudaStream_t)stream, tq, tk, tv, p));
+        if (!cfg_h) { DM_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM)); cfg_h = true; }
+        DM_CHECK_CUDA(dm_launch(attention_kernel<__half>, grid, dim3(ATT_THREADS), (size_t)ATT_SMEM, (cudaStream_t)stream, tq, tk, tv, p));
     }
     DM_CHECK_LAUNCH();
     return DM_OK;

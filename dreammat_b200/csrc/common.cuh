@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the dreammat_b200 CUDA sources (sm_100a only).
+// common.cuh -- shared helpers for the dreammat_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -8,11 +8,19 @@
 #include "../../include/dreammat_b200.h"
 
 #ifndef DM_NUM_SMS
-#define DM_NUM_SMS 148
+#define DM_NUM_SMS 132   // H100 SXM
 #endif
 
 void dm_set_error(const char* fmt, ...);
 void dm_count_launch();
+
+// Library-owned device scratch of the deterministic reductions (GroupNorm partial rows, the hash-grid backward's fixed-point
+// accumulator): one buffer per device and slot, zero-filled when allocated.  Callers of one device must not use a slot from
+// two streams at once (the same rule as the split-K workspace).  A buffer is never freed, because a captured CUDA graph may
+// hold its address; it can only grow outside stream capture (a warm-up call before capture sizes it).  Returns nullptr with
+// the error set on failure.
+enum { DM_SCRATCH_GN = 0, DM_SCRATCH_HASHGRID = 1, DM_SCRATCH_AA = 2, DM_SCRATCH_SLOTS = 3 };
+void* dm_scratch(int slot, size_t bytes, cudaStream_t st);
 
 #define DM_CHECK_CUDA(expr)                                                          \
     do {                                                                             \
@@ -25,7 +33,7 @@ void dm_count_launch();
 
 // ---- programmatic dependent launch (PDL).  Kernels of the dense section call griddep_launch_dependents() first
 // thing (the next kernel of the stream may then be scheduled as SM resources free up and run its prologue: barrier
-// init, TMEM allocation, tensor-map prefetch) and griddep_wait() before touching global memory written by earlier
+// init, tensor-map prefetch) and griddep_wait() before touching global memory written by earlier
 // kernels (it returns once every prerequisite grid has completed and flushed).  Both are no-ops for launches without
 // the attribute, so correctness never depends on the knob (dm_tune "pdl").
 extern int g_dm_pdl;

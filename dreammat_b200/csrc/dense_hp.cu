@@ -1,7 +1,7 @@
 // dense_hp.cu -- the fp32-storage ("high precision") mode of the dense path.
 //
 // The reference can run its diffusion networks with fp32 weights (half_precision_weights=false,
-// models/guidance/dreammat_guidance.py:56,92-94; BASELINE config 1 is that mode).  tcgen05 has no fp32 MMA,
+// models/guidance/dreammat_guidance.py:56,92-94; BASELINE config 1 is that mode).  the tensor cores have no fp32 MMA,
 // so the contractions keep running on the bf16 tensor-core kernel of tc_gemm.cu with BOTH operands split into
 // three bf16 terms (x = x1 + x2 + x3, 24 mantissa bits) and the six significant partial products laid side by
 // side along K:

@@ -74,20 +74,63 @@ __device__ __forceinline__ GnIdx gn_index(int HW, int vslab, int chunks) {
     return m;
 }
 
-// stats[(img*G + g)*2 + {0,1}] += (sum, sumsq) over the group's channels and the pixel chunk.  Channel PAIRS never
-// straddle a group (cpg is even for every SD layer), so each thread keeps 4 (sum, sumsq) pairs.
+// Deterministic statistics: every block reduces its threads' (a, b) pairs per group in a fixed order (no shared- or
+// global-memory float atomics) and stores them in its own row of the partials (library scratch):
+// partial[((img*slabs + slab)*chunks + chunk)*2G + 2g + {0,1}].  gn_finish_kernel then adds the rows of each group in
+// (slab, chunk) order into the caller's stats[n_img*G*2], so the statistics are bit-identical from run to run.
+__device__ __forceinline__ void gn_block_partials(const float (&a)[4], const float (&b)[4], bool active, int vslab, int cpg, int G,
+                                                  int chunks, float* __restrict__ part) {
+    __shared__ float red[256][8];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { red[threadIdx.x][2 * j] = active ? a[j] : 0.f; red[threadIdx.x][2 * j + 1] = active ? b[j] : 0.f; }
+    __syncthreads();
+    const int img = blockIdx.y, slabs = gridDim.z;
+    const int g0 = (8 * (int)blockIdx.z * vslab) / cpg, g1 = (8 * ((int)blockIdx.z + 1) * vslab - 1) / cpg;
+    float* row = part + (((int64_t)img * slabs + blockIdx.z) * chunks + blockIdx.x) * 2 * G;
+    for (int i = threadIdx.x; i < 2 * (g1 - g0 + 1); i += blockDim.x) {
+        const int g = g0 + (i >> 1), which = i & 1;
+        // threads t = q * vslab + (v - slab start) hold channel vector v; the group's vectors are [vlo, vhi] within this slab
+        const int zb = (int)blockIdx.z * vslab;
+        const int vlo = max((g * cpg) / 8, zb), vhi = min(((g + 1) * cpg - 1) / 8, zb + vslab - 1);
+        float acc = 0.f;
+        for (int q = 0; q < (int)blockDim.x / vslab; ++q)
+            for (int v = vlo; v <= vhi; ++v) {
+                const int t = q * vslab + (v - zb);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int c = 8 * v + 2 * j;         // channel pair c, c + 1 (pairs never straddle a group)
+                    if (c >= g * cpg && c < (g + 1) * cpg) acc += red[t][2 * j + which];
+                }
+            }
+        row[2 * g + which] = acc;
+    }
+}
+
+__global__ void __launch_bounds__(256) gn_finish_kernel(int n_img, int C, int G, int vslab, int slabs, int chunks,
+                                                        const float* __restrict__ part, float* __restrict__ stats) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_img * G * 2) return;
+    const int img = i / (2 * G), r = i - img * 2 * G, g = r >> 1, cpg = C / G;
+    const int z0 = ((g * cpg) / 8) / vslab, z1 = (((g + 1) * cpg - 1) / 8) / vslab;
+    float acc = 0.f;
+    for (int z = z0; z <= z1; ++z)
+        for (int c = 0; c < chunks; ++c) acc += part[(((int64_t)img * slabs + z) * chunks + c) * 2 * G + r];
+    stats[i] = acc;
+}
+
+// stats[(img*G + g)*2 + {0,1}] = (sum, sumsq) over the group's channels: this kernel writes the chunk's partial row.  Channel
+// PAIRS never straddle a group (cpg is even for every SD layer), so each thread keeps 4 (sum, sumsq) pairs.
 template <typename T>
 __global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, int HW, int C, int ld, int G,
-                                                       int chunks, int vslab, float* __restrict__ stats) {
-    extern __shared__ float s_acc[];  // [G*2]
+                                                       int chunks, int vslab, float* __restrict__ part) {
     const int img = blockIdx.y, cpg = C / G;
     griddep_launch_dependents();
-    for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) s_acc[i] = 0.f;
-    __syncthreads();
     griddep_wait();
     const GnIdx m = gn_index(HW, vslab, chunks);
+    float s[4] = {0, 0, 0, 0}, ss[4] = {0, 0, 0, 0};
     if (m.active) {
-        float s[4] = {0, 0, 0, 0}, ss[4] = {0, 0, 0, 0};
         const T* base = x + ((int64_t)img * HW) * ld + 8 * m.v;
         const int lanes = m.lanes;
         auto acc = [&](const uint4& u) {
@@ -107,16 +150,8 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, 
             for (int k = 0; k < 4; ++k) acc(u[k]);
         }
         for (; p < m.p1; p += lanes) acc(*reinterpret_cast<const uint4*>(base + (int64_t)p * ld));
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            int g = (8 * m.v + 2 * j) / cpg;
-            atomicAdd(&s_acc[2 * g], s[j]); atomicAdd(&s_acc[2 * g + 1], ss[j]);
-        }
     }
-    __syncthreads();
-    // only the groups this slab touches
-    const int g0 = (8 * (int)blockIdx.z * vslab) / cpg, g1 = (8 * ((int)blockIdx.z + 1) * vslab - 1) / cpg;
-    for (int i = 2 * g0 + threadIdx.x; i <= 2 * g1 + 1; i += blockDim.x) atomicAdd(stats + ((int64_t)img * G) * 2 + i, s_acc[i]);
+    gn_block_partials(s, ss, m.active, vslab, cpg, G, chunks, part);
 }
 
 // y = act(x * A[c] + B[c]) with A = rstd*gamma, B = beta - mean*rstd*gamma (16 registers per thread).
@@ -169,25 +204,23 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
     for (; p < m.p1; p += lanes) body(*reinterpret_cast<const uint4*>(xb + (int64_t)p * ld), p);
 }
 
-// backward pass 1: bstats[(img*G+g)*2] += sum(gamma*dy'), += sum(gamma*dy'*xhat), dy' = dz * act'(y)
+// backward pass 1: bstats[(img*G+g)*2] = sum(gamma*dy'), sum(gamma*dy'*xhat), dy' = dz * act'(y) (partial rows, as above)
 template <typename T>
 __global__ void __launch_bounds__(256) gn_bwd_stats_kernel(const T* __restrict__ x, const T* __restrict__ dz, int HW,
                                                            int C, int G, int chunks, int vslab,
                                                            const float* __restrict__ stats, const T* __restrict__ gamma,
                                                            const T* __restrict__ beta, float eps, int silu,
-                                                           float* __restrict__ bstats) {
-    extern __shared__ float s_acc[];
+                                                           float* __restrict__ part) {
     griddep_launch_dependents();
     const int img = blockIdx.y, cpg = C / G;
-    for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) s_acc[i] = 0.f;
-    __syncthreads();
     griddep_wait();
     const float inv_cnt = 1.0f / ((float)HW * (float)cpg);
     const GnIdx m = gn_index(HW, vslab, chunks);
+    float a1[4] = {0, 0, 0, 0}, a2[4] = {0, 0, 0, 0};
     if (m.active) {
         const int v = m.v, lanes = m.lanes;
         // xhat*gamma + beta = x*A + Bc;  xhat = x*rs + ms
-        float A[8], Bc[8], gm[8], rs[4], ms[4], a1[4] = {0, 0, 0, 0}, a2[4] = {0, 0, 0, 0};
+        float A[8], Bc[8], gm[8], rs[4], ms[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             int g = (8 * v + 2 * j) / cpg;
@@ -224,15 +257,8 @@ __global__ void __launch_bounds__(256) gn_bwd_stats_kernel(const T* __restrict__
         }
         for (; p < m.p1; p += lanes)
             acc(*reinterpret_cast<const uint4*>(x + base + (int64_t)p * C), *reinterpret_cast<const uint4*>(dz + base + (int64_t)p * C));
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            int g = (8 * v + 2 * j) / cpg;
-            atomicAdd(&s_acc[2 * g], a1[j]); atomicAdd(&s_acc[2 * g + 1], a2[j]);
-        }
     }
-    __syncthreads();
-    const int g0 = (8 * (int)blockIdx.z * vslab) / cpg, g1 = (8 * ((int)blockIdx.z + 1) * vslab - 1) / cpg;
-    for (int i = 2 * g0 + threadIdx.x; i <= 2 * g1 + 1; i += blockDim.x) atomicAdd(bstats + ((int64_t)img * G) * 2 + i, s_acc[i]);
+    gn_block_partials(a1, a2, m.active, vslab, cpg, G, chunks, part);
 }
 
 // backward pass 2: dx = rstd * (gamma*dy' - (S1 + xhat*S2)/cnt)  (+ dx_add if given); same mapping as gn_apply
@@ -648,6 +674,13 @@ inline int gn_chunks(int n_img, int HW, int slabs, int lanes) {
 
 }  // namespace
 
+// partial rows of one GroupNorm call in the library scratch (at least 1 MB, so one allocation serves every layer of a model)
+static float* gn_partials(int n_img, int G, int slabs, int chunks, cudaStream_t st) {
+    size_t bytes = (size_t)2 * n_img * G * slabs * chunks * sizeof(float);
+    if (bytes < ((size_t)1 << 20)) bytes = (size_t)1 << 20;
+    return (float*)dm_scratch(DM_SCRATCH_GN, bytes, st);
+}
+
 extern "C" int dm_groupnorm(int bf16, const void* x, int n_img, int HW, int C, int ld, int G, const void* gamma,
                             const void* beta, float eps, int silu, void* y, int ldy, float* stats, void* stream) {
     DM_DTYPE_OK(bf16);
@@ -655,11 +688,15 @@ extern "C" int dm_groupnorm(int bf16, const void* x, int n_img, int HW, int C, i
     DM_REQUIRE(x && gamma && beta && y && stats, "null pointer");
     DM_REQUIRE(C % 8 == 0 && C % G == 0 && (C / G) % 2 == 0 && ld % 8 == 0 && ldy % 8 == 0, "channel layout");
     cudaStream_t st = (cudaStream_t)stream;
-    DM_CHECK_CUDA(cudaMemsetAsync(stats, 0, sizeof(float) * 2 * n_img * G, st));
     const int vslab = gn_vslab(C / 8), slabs = (C / 8) / vslab;
     const int chunks = gn_chunks(n_img, HW, slabs, 256 / vslab);
     const dim3 grid(chunks, n_img, slabs);
-    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_stats_kernel<T>, grid, dim3(256), 2 * G * sizeof(float), st, (const T*)x, HW, C, ld, G, chunks, vslab, stats)));
+    float* part = gn_partials(n_img, G, slabs, chunks, st);
+    if (!part) return DM_EDRIVER;
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_stats_kernel<T>, grid, dim3(256), 0, st, (const T*)x, HW, C, ld, G, chunks, vslab, part)));
+    DM_CHECK_LAUNCH();
+    DM_CHECK_CUDA(dm_launch(gn_finish_kernel, dim3((unsigned)dm_ceil_div(2 * n_img * G, 256)), dim3(256), 0, st, n_img, C, G, vslab, slabs, chunks,
+                            (const float*)part, stats));
     DM_CHECK_LAUNCH();
     DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_apply_kernel<T>, grid, dim3(256), 0, st, (const T*)x, HW, C, ld, ldy, G, chunks, vslab, (const float*)stats,
                                                 (const T*)gamma, (const T*)beta, eps, silu, (T*)y)));
@@ -675,12 +712,16 @@ extern "C" int dm_groupnorm_bwd(int bf16, const void* x, const void* dz, int n_i
     DM_REQUIRE(x && dz && gamma && beta && stats && bstats && dx, "null pointer");
     DM_REQUIRE(C % 8 == 0 && C % G == 0 && (C / G) % 2 == 0, "channel layout");
     cudaStream_t st = (cudaStream_t)stream;
-    DM_CHECK_CUDA(cudaMemsetAsync(bstats, 0, sizeof(float) * 2 * n_img * G, st));
     const int vslab = gn_vslab(C / 8), slabs = (C / 8) / vslab;
     const int chunks = gn_chunks(n_img, HW, slabs, 256 / vslab);
     const dim3 grid(chunks, n_img, slabs);
-    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_bwd_stats_kernel<T>, grid, dim3(256), 2 * G * sizeof(float), st,
-                            (const T*)x, (const T*)dz, HW, C, G, chunks, vslab, stats, (const T*)gamma, (const T*)beta, eps, silu, bstats)));
+    float* part = gn_partials(n_img, G, slabs, chunks, st);
+    if (!part) return DM_EDRIVER;
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_bwd_stats_kernel<T>, grid, dim3(256), 0, st,
+                            (const T*)x, (const T*)dz, HW, C, G, chunks, vslab, stats, (const T*)gamma, (const T*)beta, eps, silu, part)));
+    DM_CHECK_LAUNCH();
+    DM_CHECK_CUDA(dm_launch(gn_finish_kernel, dim3((unsigned)dm_ceil_div(2 * n_img * G, 256)), dim3(256), 0, st, n_img, C, G, vslab, slabs, chunks,
+                            (const float*)part, bstats));
     DM_CHECK_LAUNCH();
     DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_bwd_apply_kernel<T>, grid, dim3(256), 0, st, (const T*)x, (const T*)dz, HW, C, G, chunks, vslab, stats,
                                                 (const float*)bstats, (const T*)gamma, (const T*)beta, eps, silu, (const T*)dx_add, (T*)dx)));

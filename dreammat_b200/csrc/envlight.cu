@@ -6,7 +6,7 @@
 // GGX-prefiltered specular mips (roughness 0.08 .. 0.5 linearly over the chain, 1.0 for the last) and a
 // cosine-convolved diffuse cube at 16^2.  `shade_splitsum` (:679-711) then needs only three texture lookups per pixel.
 // Here the same construction runs as four small kernels (fp32, brute-force texel-pair sums: 6*128^2 squared is 9.7e9
-// pairs, tens of milliseconds on a B200); dreammat_b200/envlight.py drives them and caches the result on disk.
+// pairs, tens of milliseconds on the GPU); dreammat_b200/envlight.py drives them and caches the result on disk.
 #include "common.cuh"
 
 namespace {

@@ -7,11 +7,14 @@
 // Parameter layout is tiny-cuda-nn's (level-major, entry-major, features interleaved) so a
 // reference checkpoint's `geometry.encoding.encoding.encoding.params` loads unchanged.
 //
-// Memory behaviour: the 50.4 MB table is L2-resident on B200 (126 MB L2); each point does
+// Memory behaviour: the 50.4 MB table is about the size of the H100's 50 MB L2; each point does
 // 16 levels x 8 corner float2 gathers.  One thread owns (point, 4 levels) in the gather phase
 // so 32 independent 8-byte loads are in flight per thread; the MLP runs out of shared memory.
-// Backward recomputes the forward (nothing saved), scatters with red.global.add.v2.f32 and
-// keeps the weight gradients in shared memory until the block retires.
+// Backward recomputes the forward (nothing saved) and is deterministic: the grid gradient is scattered as int64 fixed
+// point into a library-owned accumulator (integer adds are associative, so the order in which warps arrive does not change
+// the sum) with a power-of-two scale fixed per call from a bound on every finite contribution; one pass then adds it to
+// dgrid in fp32.  Non-finite contributions go straight to dgrid (inf / nan results do not depend on the order).  The weight gradients
+// stay in shared memory until the block retires and are written as per-block rows that are added in block order.
 #include "common.cuh"
 
 namespace {
@@ -22,6 +25,29 @@ constexpr int NTHREADS = 256;  // 4 level-groups x 64 points
 constexpr int ENC = 32;
 constexpr int HID = 64;
 constexpr int NOUT = 5;
+
+constexpr int DW_ROW = HID * ENC + NOUT * HID;   // one block's dW1 | dW2 partial row
+constexpr int BWD_MAX_BLOCKS = DM_NUM_SMS * 2;
+constexpr int64_t HDR_BYTES = 256;
+
+// Fixed-point scale 2^e of a backward call: every contribution is at most U = hdr[0]*hdr[1]*hdr[2] in magnitude and an
+// entry receives at most 8 per point and level, so |sum| * 2^e < 8 n U 2^e <= 2^62 fits int64.
+__device__ __forceinline__ double fixed_scale(const uint32_t* hdr, int64_t n) {
+    const double U = (double)__uint_as_float(hdr[0]) * (double)__uint_as_float(hdr[1]) * (double)__uint_as_float(hdr[2]);
+    if (!(U > 0.0) || !isfinite(U)) return 1.0;
+    int eu, en;
+    frexp(U, &eu);                       // U < 2^eu
+    frexp((double)(8 * (n > 0 ? n : 1)), &en);
+    return ldexp(1.0, 62 - eu - en);
+}
+__device__ __forceinline__ void fixed_add(unsigned long long* acc, float* dgrid, int64_t i, float v, double S) {
+    if (v == 0.f) return;
+    const double q = (double)v * S;
+    if (isfinite(v) && fabs(q) < 4.6116860184273879e18)        // 2^62: inside the bound (always, for finite weights)
+        atomicAdd(acc + i, (unsigned long long)__double2ll_rn(q));
+    else
+        atomicAdd(dgrid + i, v);
+}
 
 struct LevelMeta {
     float scale[MAXL];
@@ -167,8 +193,10 @@ __global__ void __launch_bounds__(NTHREADS) hashgrid_bwd_kernel(LevelMeta m, con
                                                                 const float* __restrict__ W1,
                                                                 const float* __restrict__ W2,
                                                                 const float* __restrict__ dout,
-                                                                float2* __restrict__ dgrid, float* __restrict__ dW1,
-                                                                float* __restrict__ dW2) {
+                                                                const uint32_t* __restrict__ hdr,
+                                                                unsigned long long* __restrict__ acc_grid,
+                                                                float* __restrict__ dgrid, float* __restrict__ dw_part) {
+    const double S = fixed_scale(hdr, n);
     __shared__ float s_enc[TILE][ENC + 1];
     __shared__ float s_w1[HID][ENC + 1];
     __shared__ float s_w2[NOUT][HID];
@@ -288,7 +316,7 @@ __global__ void __launch_bounds__(NTHREADS) hashgrid_bwd_kernel(LevelMeta m, con
                                 // lane + d belongs to this lane's run iff no head lies in (lane, lane + d]
                                 if (lane + d < 32 && (after & ((1u << d) - 1u)) == 0u) { v0 += o0; v1 += o1; }
                             }
-                            if (head && idx != 0xffffffffu) atomicAdd(dgrid + idx, make_float2(v0, v1));
+                            if (head && idx != 0xffffffffu) { fixed_add(acc_grid, dgrid, 2 * (int64_t)idx, v0, S); fixed_add(acc_grid, dgrid, 2 * (int64_t)idx + 1, v1, S); }
                         }
                     }
                 }
@@ -301,15 +329,64 @@ __global__ void __launch_bounds__(NTHREADS) hashgrid_bwd_kernel(LevelMeta m, con
                         level_corners(m, l, x, y, z, c);
                         float g0 = acc[2 * j], g1 = acc[2 * j + 1];
 #pragma unroll
-                        for (int k = 0; k < 8; ++k) atomicAdd(dgrid + c.idx[k], make_float2(c.w[k] * g0, c.w[k] * g1));
+                        for (int k = 0; k < 8; ++k) { fixed_add(acc_grid, dgrid, 2 * (int64_t)c.idx[k], c.w[k] * g0, S); fixed_add(acc_grid, dgrid, 2 * (int64_t)c.idx[k] + 1, c.w[k] * g1, S); }
                     }
                 }
             }
         }
     }
     __syncthreads();
-    for (int i = tid; i < HID * ENC; i += NTHREADS) atomicAdd(dW1 + i, s_dw1[i / ENC][i % ENC]);
-    for (int i = tid; i < NOUT * HID; i += NTHREADS) atomicAdd(dW2 + i, s_dw2[i / HID][i % HID]);
+    float* row = dw_part + (int64_t)blockIdx.x * DW_ROW;
+    for (int i = tid; i < HID * ENC; i += NTHREADS) row[i] = s_dw1[i / ENC][i % ENC];
+    for (int i = tid; i < NOUT * HID; i += NTHREADS) row[HID * ENC + i] = s_dw2[i / HID][i % HID];
+}
+
+// bound of every finite grid-gradient contribution c.w * denc (c.w <= 1): |denc_k| <= |dout_p|_1 * max|W2| * sum_h |W1[h][k]|
+// (non-finite entries are left out: their contributions take the direct path of fixed_add).
+// hdr[0] = max_p |dout_p|_1, hdr[1] = max|W2|, hdr[2] = max_k sum_h |W1[h][k]| (float bits; non-negative floats order like
+// their bit patterns, so atomicMax on them is exact and order-independent).  hdr[0] is zeroed by the host first.
+__global__ void __launch_bounds__(256) hashgrid_bound_kernel(const float* __restrict__ dout, int64_t n, const float* __restrict__ W1,
+                                                             const float* __restrict__ W2, uint32_t* __restrict__ hdr) {
+    float mx = 0.f;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
+        float a = 0.f;
+#pragma unroll
+        for (int c = 0; c < NOUT; ++c) { const float d = fabsf(dout[p * NOUT + c]); if (isfinite(d)) a += d; }
+        if (isfinite(a)) mx = fmaxf(mx, a);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(hdr, __float_as_uint(mx));
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        float w2 = 0.f, w1 = 0.f;
+        for (int i = 0; i < NOUT * HID; ++i) if (isfinite(W2[i])) w2 = fmaxf(w2, fabsf(W2[i]));
+        for (int k = 0; k < ENC; ++k) {
+            float c = 0.f;
+            for (int h = 0; h < HID; ++h) if (isfinite(W1[h * ENC + k])) c += fabsf(W1[h * ENC + k]);
+            if (isfinite(c)) w1 = fmaxf(w1, c);
+        }
+        hdr[1] = __float_as_uint(w2); hdr[2] = __float_as_uint(w1);
+    }
+}
+
+// dgrid += fixed-point sums / S, and the accumulator goes back to zero for the next call
+__global__ void __launch_bounds__(256) hashgrid_fixed_flush_kernel(const uint32_t* __restrict__ hdr, int64_t n, int64_t count,
+                                                                   unsigned long long* __restrict__ acc_grid, float* __restrict__ dgrid) {
+    const double inv = 1.0 / fixed_scale(hdr, n);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
+        const unsigned long long v = acc_grid[i];
+        if (v) { dgrid[i] += (float)((double)(long long)v * inv); acc_grid[i] = 0ull; }
+    }
+}
+
+// dW1 | dW2 += the blocks' rows, in block order
+__global__ void __launch_bounds__(256) hashgrid_dw_reduce_kernel(const float* __restrict__ dw_part, int blocks, float* __restrict__ dW1,
+                                                                 float* __restrict__ dW2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= DW_ROW) return;
+    float a = 0.f;
+    for (int b = 0; b < blocks; ++b) a += dw_part[(int64_t)b * DW_ROW + i];
+    if (i < HID * ENC) dW1[i] += a; else dW2[i - HID * ENC] += a;
 }
 
 }  // namespace
@@ -364,12 +441,25 @@ extern "C" int dm_hashgrid_mlp_bwd(const dm_hashgrid_cfg* cfg, const float* poin
                                    float* dW2, void* stream) {
     if (n == 0) return DM_OK;
     DM_REQUIRE(cfg && points && grid && W1 && W2 && dfeatures && dgrid && dW1 && dW2, "null pointer");
-    LevelMeta m; int rc = make_meta(cfg, m, nullptr); if (rc) return rc;
+    LevelMeta m; int64_t total = 0; int rc = make_meta(cfg, m, &total); if (rc) return rc;
     rc = check_mlp(cfg); if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    // header | per-block weight-gradient rows | int64 accumulator [total * 2] (zero between calls: the flush re-zeroes it)
+    void* scratch = dm_scratch(DM_SCRATCH_HASHGRID, (size_t)(HDR_BYTES + (int64_t)BWD_MAX_BLOCKS * DW_ROW * 4 + total * 2 * 8), st);
+    if (!scratch) return DM_EDRIVER;
+    uint32_t* hdr = (uint32_t*)scratch;
+    float* dw_part = (float*)((char*)scratch + HDR_BYTES);
+    unsigned long long* acc_grid = (unsigned long long*)((char*)scratch + HDR_BYTES + (int64_t)BWD_MAX_BLOCKS * DW_ROW * 4);
     int64_t tiles = dm_ceil_div(n, TILE);
-    int grid_dim = (int)(tiles < (int64_t)DM_NUM_SMS * 2 ? tiles : (int64_t)DM_NUM_SMS * 2);
-    hashgrid_bwd_kernel<<<grid_dim, NTHREADS, 0, (cudaStream_t)stream>>>(m, points, n, (const float2*)grid, W1, W2, dfeatures,
-                                                                          (float2*)dgrid, dW1, dW2);
+    int grid_dim = (int)(tiles < (int64_t)BWD_MAX_BLOCKS ? tiles : (int64_t)BWD_MAX_BLOCKS);
+    DM_CHECK_CUDA(cudaMemsetAsync(hdr, 0, 4, st));
+    hashgrid_bound_kernel<<<(unsigned)(dm_ceil_div(n, 256) < DM_NUM_SMS * 4 ? dm_ceil_div(n, 256) : DM_NUM_SMS * 4), 256, 0, st>>>(dfeatures, n, W1, W2, hdr);
+    DM_CHECK_LAUNCH();
+    hashgrid_bwd_kernel<<<grid_dim, NTHREADS, 0, st>>>(m, points, n, (const float2*)grid, W1, W2, dfeatures, hdr, acc_grid, dgrid, dw_part);
+    DM_CHECK_LAUNCH();
+    hashgrid_dw_reduce_kernel<<<(unsigned)dm_ceil_div(DW_ROW, 256), 256, 0, st>>>(dw_part, grid_dim, dW1, dW2);
+    DM_CHECK_LAUNCH();
+    hashgrid_fixed_flush_kernel<<<DM_NUM_SMS * 8, 256, 0, st>>>(hdr, n, total * 2, acc_grid, dgrid);
     DM_CHECK_LAUNCH();
     return DM_OK;
 }

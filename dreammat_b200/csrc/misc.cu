@@ -1,5 +1,7 @@
 // misc.cu -- error plumbing, compaction / canvas scatter (a2, a6), Adam (a9), CSD combine (a8 tail).
 #include <stdarg.h>
+#include <map>
+#include <mutex>
 #include <vector>
 #include "common.cuh"
 
@@ -19,13 +21,37 @@ void dm_count_launch() { __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED); }
 extern "C" long long dm_launch_count(void) { return __atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
 
 extern "C" const char* dm_last_error(void) { return g_err; }
+
+void* dm_scratch(int slot, size_t bytes, cudaStream_t st) {
+    struct Buf { void* p; size_t bytes; };
+    static std::mutex mu;
+    static std::map<std::pair<int, int>, Buf> bufs;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) { dm_set_error("dm_scratch: no current device"); return nullptr; }
+    std::lock_guard<std::mutex> lock(mu);
+    Buf& b = bufs[{dev, slot}];
+    if (b.p && b.bytes >= bytes) return b.p;
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(st, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone) {
+        dm_set_error("library scratch (slot %d) must grow to %zu bytes while the stream is being captured: run the same call once "
+                     "before capture", slot, bytes);
+        return nullptr;
+    }
+    void* p = nullptr;
+    if (cudaMalloc(&p, bytes) != cudaSuccess || cudaMemsetAsync(p, 0, bytes, st) != cudaSuccess) {
+        dm_set_error("library scratch: cudaMalloc / memset of %zu bytes failed", bytes);
+        return nullptr;
+    }
+    b.p = p; b.bytes = bytes;      // the old buffer (if any) stays allocated: a captured graph may still use it
+    return p;
+}
 extern "C" int dm_version(void) { return 100; }
 
 extern "C" int dm_device_check(int dev) {
     cudaDeviceProp p;
     DM_CHECK_CUDA(cudaGetDeviceProperties(&p, dev));
-    if (p.major != 10) {
-        dm_set_error("device %d is sm_%d%d; this library only carries sm_100a code", dev, p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) {
+        dm_set_error("device %d is sm_%d%d; this library only carries sm_90a code", dev, p.major, p.minor);
         return DM_EUNSUPPORTED;
     }
     return DM_OK;
@@ -132,24 +158,103 @@ __global__ void __launch_bounds__(256) adam_kernel(float4* __restrict__ p, const
     if (i < tail) upd(pt[i], gt[i], mt[i], vt[i]);
 }
 
-// silhouette antialias as a cached sparse blend (see dreammat_b200/antialias.py): out[dst] += a * (in[src] - in[dst])
-__global__ void aa_fwd_kernel(const float* __restrict__ in, const int32_t* __restrict__ dst, const int32_t* __restrict__ src,
-                              const float* __restrict__ alpha, int64_t k, int c, float* __restrict__ out) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= k * c) return;
-    int64_t e = i / c; int ch = (int)(i - e * c);
-    int64_t d = dst[e], s_ = src[e];
-    atomicAdd(out + d * c + ch, alpha[e] * (in[s_ * c + ch] - in[d * c + ch]));
+// silhouette antialias as a cached sparse blend (see dreammat_b200/antialias.py): out[dst] += a * (in[src] - in[dst]).
+// Deterministic for any pair order, O(k): each pair drops its index into a small bucket of its key pixel (library scratch:
+// count[n_pix] + AA_CAP slots per pixel); the pair with the lowest index owns the pixel and sums the bucket's pairs in index
+// order (a fuller bucket falls back to a scan of the list); a last pass clears the touched counts.  No fp32 atomics.
+constexpr int AA_CAP = 8;
+__global__ void aa_bucket_kernel(const int32_t* __restrict__ key, int64_t k, int32_t* __restrict__ cnt, int32_t* __restrict__ slot) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= k) return;
+    const int64_t x = key[e];
+    const int i = atomicAdd(cnt + x, 1);
+    if (i < AA_CAP) slot[x * AA_CAP + i] = (int32_t)e;
 }
-__global__ void aa_bwd_kernel(const float* __restrict__ dout, const int32_t* __restrict__ dst, const int32_t* __restrict__ src,
-                              const float* __restrict__ alpha, int64_t k, int c, float* __restrict__ din) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= k * c) return;
-    int64_t e = i / c; int ch = (int)(i - e * c);
-    int64_t d = dst[e], s_ = src[e];
-    float g = alpha[e] * dout[d * c + ch];
-    atomicAdd(din + s_ * c + ch, g);
-    atomicAdd(din + d * c + ch, -g);
+__global__ void aa_clear_kernel(const int32_t* __restrict__ key, int64_t k, int32_t* __restrict__ cnt) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < k) cnt[key[e]] = 0;
+}
+// pairs of pixel key[e] in index order if e owns the pixel (returns their number; -1: e owns it but the bucket overflowed,
+// scan the list from e), 0 if another pair owns it
+__device__ __forceinline__ int aa_owned(const int32_t* __restrict__ key, int64_t e, const int32_t* __restrict__ cnt,
+                                        const int32_t* __restrict__ slot, int32_t (&list)[AA_CAP]) {
+    const int64_t x = key[e];
+    const int c = cnt[x];
+    if (c > AA_CAP) {
+        for (int64_t j = 0; j < e; ++j) if (key[j] == x) return 0;
+        return -1;
+    }
+    for (int i = 0; i < c; ++i) {
+        const int32_t v = slot[x * AA_CAP + i];
+        if (v < e) return 0;
+        int p = i;                                  // insertion sort (c <= 8)
+        while (p > 0 && list[p - 1] > v) { list[p] = list[p - 1]; --p; }
+        list[p] = v;
+    }
+    return c;
+}
+__global__ void aa_fwd_kernel(const float* __restrict__ in, const int32_t* __restrict__ dst, const int32_t* __restrict__ src,
+                              const float* __restrict__ alpha, int64_t k, int c, const int32_t* __restrict__ cnt,
+                              const int32_t* __restrict__ slot, float* __restrict__ out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= k) return;
+    int32_t list[AA_CAP];
+    const int m = aa_owned(dst, e, cnt, slot, list);
+    if (m == 0) return;
+    const int64_t d = dst[e];
+    for (int ch = 0; ch < c; ++ch) {
+        const float base = in[d * c + ch];
+        float acc = 0.f;
+        if (m > 0) {
+            for (int i = 0; i < m; ++i) acc += alpha[list[i]] * (in[(int64_t)src[list[i]] * c + ch] - base);
+        } else {
+            for (int64_t j = e; j < k; ++j) if (dst[j] == d) acc += alpha[j] * (in[(int64_t)src[j] * c + ch] - base);
+        }
+        out[d * c + ch] = base + acc;
+    }
+}
+// adjoint, pass 1 (destination side): din[dst] -= sum a * dout[dst]
+__global__ void aa_bwd_dst_kernel(const float* __restrict__ dout, const int32_t* __restrict__ dst, const float* __restrict__ alpha,
+                                  int64_t k, int c, const int32_t* __restrict__ cnt, const int32_t* __restrict__ slot,
+                                  float* __restrict__ din) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= k) return;
+    int32_t list[AA_CAP];
+    const int m = aa_owned(dst, e, cnt, slot, list);
+    if (m == 0) return;
+    const int64_t d = dst[e];
+    float a = 0.f;
+    if (m > 0) { for (int i = 0; i < m; ++i) a += alpha[list[i]]; }
+    else { for (int64_t j = e; j < k; ++j) if (dst[j] == d) a += alpha[j]; }
+    for (int ch = 0; ch < c; ++ch) din[d * c + ch] -= a * dout[d * c + ch];
+}
+// adjoint, pass 2 (source side, after pass 1): din[src] += sum a * dout[dst]
+__global__ void aa_bwd_src_kernel(const float* __restrict__ dout, const int32_t* __restrict__ dst, const int32_t* __restrict__ src,
+                                  const float* __restrict__ alpha, int64_t k, int c, const int32_t* __restrict__ cnt,
+                                  const int32_t* __restrict__ slot, float* __restrict__ din) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= k) return;
+    int32_t list[AA_CAP];
+    const int m = aa_owned(src, e, cnt, slot, list);
+    if (m == 0) return;
+    const int64_t s_ = src[e];
+    for (int ch = 0; ch < c; ++ch) {
+        float acc = 0.f;
+        if (m > 0) {
+            for (int i = 0; i < m; ++i) acc += alpha[list[i]] * dout[(int64_t)dst[list[i]] * c + ch];
+        } else {
+            for (int64_t j = e; j < k; ++j) if (src[j] == s_) acc += alpha[j] * dout[(int64_t)dst[j] * c + ch];
+        }
+        din[s_ * c + ch] += acc;
+    }
+}
+
+// bucket scratch of one antialias call: count[n_pix] then AA_CAP slots per pixel (counts are zero between calls)
+static int aa_scratch(int64_t n_pix, cudaStream_t st, int32_t** cnt, int32_t** slot) {
+    void* p = dm_scratch(DM_SCRATCH_AA, (size_t)n_pix * (1 + AA_CAP) * sizeof(int32_t), st);
+    if (!p) return DM_EDRIVER;
+    *cnt = (int32_t*)p; *slot = *cnt + n_pix;
+    return DM_OK;
 }
 
 // F.interpolate(mode="bilinear", align_corners=False) on NHWC fp32 (dreammat_guidance.py:507-513) and its adjoint
@@ -278,7 +383,13 @@ extern "C" int dm_antialias_fwd(const float* in, const int32_t* dst, const int32
     if (in != out) DM_CHECK_CUDA(cudaMemcpyAsync(out, in, sizeof(float) * n_pix * c, cudaMemcpyDeviceToDevice, st));
     if (k == 0) return DM_OK;
     DM_REQUIRE(dst && src && alpha && in != out, "null pointer / in-place with pairs");
-    aa_fwd_kernel<<<(unsigned)dm_ceil_div(k * c, 256), 256, 0, st>>>(in, dst, src, alpha, k, c, out);
+    int32_t *cnt, *slot; int rc = aa_scratch(n_pix, st, &cnt, &slot); if (rc) return rc;
+    const unsigned blocks = (unsigned)dm_ceil_div(k, 128);
+    aa_bucket_kernel<<<blocks, 128, 0, st>>>(dst, k, cnt, slot);
+    DM_CHECK_LAUNCH();
+    aa_fwd_kernel<<<blocks, 128, 0, st>>>(in, dst, src, alpha, k, c, cnt, slot, out);
+    DM_CHECK_LAUNCH();
+    aa_clear_kernel<<<blocks, 128, 0, st>>>(dst, k, cnt);
     DM_CHECK_LAUNCH();
     return DM_OK;
 }
@@ -290,7 +401,19 @@ extern "C" int dm_antialias_bwd(const float* dout, const int32_t* dst, const int
     DM_CHECK_CUDA(cudaMemcpyAsync(din, dout, sizeof(float) * n_pix * c, cudaMemcpyDeviceToDevice, st));
     if (k == 0) return DM_OK;
     DM_REQUIRE(dst && src && alpha, "null pointer");
-    aa_bwd_kernel<<<(unsigned)dm_ceil_div(k * c, 256), 256, 0, st>>>(dout, dst, src, alpha, k, c, din);
+    int32_t *cnt, *slot; int rc = aa_scratch(n_pix, st, &cnt, &slot); if (rc) return rc;
+    const unsigned blocks = (unsigned)dm_ceil_div(k, 128);
+    aa_bucket_kernel<<<blocks, 128, 0, st>>>(dst, k, cnt, slot);
+    DM_CHECK_LAUNCH();
+    aa_bwd_dst_kernel<<<blocks, 128, 0, st>>>(dout, dst, alpha, k, c, cnt, slot, din);
+    DM_CHECK_LAUNCH();
+    aa_clear_kernel<<<blocks, 128, 0, st>>>(dst, k, cnt);
+    DM_CHECK_LAUNCH();
+    aa_bucket_kernel<<<blocks, 128, 0, st>>>(src, k, cnt, slot);
+    DM_CHECK_LAUNCH();
+    aa_bwd_src_kernel<<<blocks, 128, 0, st>>>(dout, dst, src, alpha, k, c, cnt, slot, din);
+    DM_CHECK_LAUNCH();
+    aa_clear_kernel<<<blocks, 128, 0, st>>>(src, k, cnt);
     DM_CHECK_LAUNCH();
     return DM_OK;
 }

@@ -8,7 +8,7 @@
 //   dm_shade_splitsum_fwd  dreammat_material.py:679-711 (shade_splitsum)
 //   dm_shade_bwd           what torch autograd does for either branch, in closed form
 //
-// Design (B200-first).  The reference materialises >= 40 tensors of shape [pn,328,{1,3}] per view
+// Design (GPU-first).  The reference materialises >= 40 tensors of shape [pn,328,{1,3}] per view
 // and keeps them for autograd.  Here one WARP owns one covered pixel: lanes stride over the 328
 // light samples, each lane builds its direction, evaluates the BRDF terms, walks the BVH for
 // occlusion (any-hit) and fetches one env-map texel; partial sums are folded with warp

@@ -1,11 +1,11 @@
-// tc_gemm.cu -- tcgen05 tensor-core GEMM / implicit-GEMM convolution for sm_100a.
+// tc_gemm.cu -- wgmma tensor-core GEMM / implicit-GEMM convolution for sm_90a.
 //
 // Every dense contraction of the VAE encoder, the UNet and the ControlNet runs through this file
 // (rows a7/a8 of SURVEY.md section 8; reference call sites models/guidance/dreammat_guidance.py:
 // 218-229 ControlNetModel.forward, :274-282 UNet2DConditionModel.forward, :290 AutoencoderKL.encode,
 // which run cuDNN/cuBLAS kernels through diffusers):
 //
-//   D[M,N] = epilogue( A[M,K] . B[N,K]^T )        fp16 or bf16 operands, fp32 accumulation in TMEM
+//   D[M,N] = epilogue( A[M,K] . B[N,K]^T )        fp16 or bf16 operands, fp32 accumulation in registers
 //
 //   * linear / 1x1 conv : A = activations [batch, M, K] through a 3-D TMA map
 //   * 3x3 conv (NHWC)   : A is never materialised (no im2col).  The K loop walks (tap, 64-channel
@@ -14,17 +14,13 @@
 //                         Stride-2 convs use the map's element strides.
 //   * B = weights [N, K] (K-major), K index = tap * Cin + c.
 //
-// Three kernels share one epilogue (epilogue_tile: tcgen05.ld -> registers -> fused bias / per-image
-// vector / residual / SiLU / GELU / GEGLU / scale -> 16-byte global stores, or fp32 red.add for split-K):
-//   tc_gemm_kernel<BN,T,CPS>      one CTA per 128 x BN tile, 1-2 persistent CTAs per SM
-//   tc_gemm_pair_kernel<BN,T>     cta_group::2: a CTA pair per 256 x BN tile (the work-horse)
-//   tc_conv_halo_kernel<BN,T,M>   experiment: halo tile re-used across the nine taps (default off)
-// CTA = 192 threads: warp 0 TMA producer, warp 1 TMEM allocator + single-thread tcgen05.mma issuer,
-// warps 2-5 epilogue.  Operand tiles live in the 128-byte swizzled K-major layout shared by TMA and
-// the UMMA descriptors; a ring of mbarrier-guarded stages feeds the tensor core, tcgen05.commit
-// releases stages and signals the epilogue; the TMEM accumulator is double-buffered so the epilogue
-// of tile i overlaps the main loop of tile i+1.  choose_tile() picks kernel, tile width and split-K
-// from measured sweeps (profiles/r01_tile_sweep.txt, r01_exp_splitk.txt).
+// tc_gemm_kernel<BN,T>: persistent, warp-specialised, one CTA per SM walking 128 x BN output tiles.  CTA = 288 threads:
+// warps 0-7 are two consumer warpgroups (rows 0-63 / 64-127 of the tile, m64nBNk16 wgmma with both operands in shared
+// memory), warp 8 is the TMA producer.  Operand tiles live in the 128-byte swizzled K-major layout shared by TMA and the
+// wgmma descriptors; a ring of mbarrier-guarded stages lets the producer run ahead across tile boundaries.  After the K
+// loop the accumulators go through a shared-memory staging tile so the epilogue (fused bias / per-image vector / residual
+// / SiLU / GELU / GEGLU / scale -> 16-byte global stores, or a split-K partial tile) reads whole output rows.
+// choose_tile() picks the tile width and split-K.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -34,7 +30,8 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int NTHREADS = 192;
+constexpr int CONSUMERS = 256;                 // two warpgroups
+constexpr int NTHREADS = CONSUMERS + 32;       // + the TMA producer warp
 
 struct GemmParams {
     int M, N, K;                  // GEMM view; conv: M = n_img*Ho*Wo, K = taps*Cin
@@ -51,7 +48,7 @@ struct GemmParams {
     float alpha;                            // applied to the accumulator first
     float out_scale;                        // applied last
     int act;                                // 0 none, 1 silu, 2 gelu(erf), 3 geglu (interleaved value|gate)
-    int split_k; float* ws;                 // split-K: fp32 partial sums are red.add'ed into ws[M, N]; splitk_finish_kernel applies the epilogue
+    int split_k; float* ws;                 // split-K: split sp stores its fp32 partial tile in slice sp of ws[S][batch][M][N]; splitk_finish_kernel sums the slices in order and applies the epilogue
     // fused CSD epilogue of the UNet's conv_out (dm_conv2d_csd): rows are [branch][view][pixel]; a CTA walks the three
     // branch tiles of the same 128 pixels back to back and combines them in registers
     int csd; int csd_B; int csd_hw; int csd_groups;       // csd_groups = B*hw / 128 row tiles per branch
@@ -77,49 +74,40 @@ template <> struct Cvt<__nv_bfloat16> {
     static __device__ __forceinline__ __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
 };
 
-// Epilogue of one 128-row accumulator tile: this warp's 32 TMEM lanes (one output row per thread), BN columns in
-// chunks of 32: acc*alpha + bias + rowvec -> act -> + residual -> * out_scale -> 16-byte stores.  `release_bar` is
-// arrived on (once per warp) as soon as the last chunk sits in registers, handing the TMEM buffer back to the MMA
-// issuer; REMOTE = the barrier lives in the leader CTA of a pair (shared::cluster address).
-// DUAL: the K loop alternated its MMAs between two accumulators (tmem_acc and tmem_acc + BN); their sum is the tile.
-template <int BN, typename T, bool REMOTE, bool DUAL = false>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tmem_acc, int64_t m, int z, int n_tile,
-                                              int lane, uint32_t release_bar) {
-    auto ld_acc = [&](uint32_t col, uint32_t (&v)[32]) {
-        tmem_ld_32x32b_x32(tmem_acc + col, v);
-        if constexpr (DUAL) {
-            uint32_t w2[32];
-            tmem_ld_32x32b_x32(tmem_acc + (uint32_t)BN + col, w2);
-            tmem_ld_wait();
+__device__ __forceinline__ void ld_row32(const float* er, int c0, float (&f)[32]) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(w2[j]));
-        }
-    };
+    for (int q = 0; q < 8; ++q) {
+        const float4 t = reinterpret_cast<const float4*>(er + c0)[q];
+        f[4 * q] = t.x; f[4 * q + 1] = t.y; f[4 * q + 2] = t.z; f[4 * q + 3] = t.w;
+    }
+}
+
+// Epilogue of one output row of a 128 x BN tile: `er` is the row's fp32 accumulator in the staging tile; this thread
+// handles the column chunks c0 = c_first, c_first + c_step, ... (32 wide, 64 for GEGLU):
+// acc*alpha + bias + rowvec -> act -> + residual -> * out_scale -> 16-byte stores.
+template <int BN, typename T>
+__device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* er, int64_t m, int z, int sp, int n_tile,
+                                             int c_first, int c_step) {
     const bool row_ok = m < p.M;
+    if (!row_ok) return;
     if (p.ws) {
-        // split-K partial tile: accumulate raw fp32 sums; the epilogue proper runs in splitk_finish_kernel
-        float* wrow = p.ws + ((int64_t)z * p.M + m) * p.N;
+        // split-K partial tile: raw fp32 sums into this split's own slice (no atomics: the finish kernel adds the slices in a
+        // fixed order, so the result does not depend on which split finishes first); the epilogue proper runs there
+        const int64_t slice = (int64_t)(p.batch > 0 ? p.batch : 1) * p.M * p.N;
+        float* wrow = p.ws + sp * slice + ((int64_t)z * p.M + m) * p.N;
 #pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            uint32_t v[32];
-            ld_acc((uint32_t)c0, v);
-            tmem_ld_wait();
-            if (c0 + 32 >= BN) {
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) { if (REMOTE) mbar_arrive_cluster(release_bar); else mbar_arrive(release_bar); }
-            }
+        for (int c0 = c_first; c0 < BN; c0 += c_step) {
             const int n0 = n_tile * BN + c0;
-            if (!row_ok || n0 >= p.N) continue;
+            if (n0 >= p.N) continue;
+            float v[32];
+            ld_row32(er, c0, v);
             if (n0 + 32 <= p.N && (p.N & 3) == 0) {
 #pragma unroll
                 for (int q = 0; q < 8; ++q)
-                    atomicAdd(reinterpret_cast<float4*>(wrow + n0) + q,
-                              make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                                          __uint_as_float(v[4 * q + 3])));
+                    reinterpret_cast<float4*>(wrow + n0)[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
             } else {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) if (n0 + j < p.N) atomicAdd(wrow + n0 + j, __uint_as_float(v[j]));
+                for (int j = 0; j < 32; ++j) if (n0 + j < p.N) wrow[n0 + j] = v[j];
             }
         }
         return;
@@ -133,18 +121,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tmem
         // dense_ops.geglu_interleave), so every 64 accumulator columns give 32 outputs value * gelu(gate)
         // and the [M, N] projection never goes to HBM.  Output row length is N / 2.
 #pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 64) {
-            uint32_t v[32], g[32];
-            ld_acc((uint32_t)c0, v);
-            ld_acc((uint32_t)(c0 + 32), g);
-            tmem_ld_wait();
-            if (c0 + 64 >= BN) {
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) { if (REMOTE) mbar_arrive_cluster(release_bar); else mbar_arrive(release_bar); }
-            }
+        for (int c0 = c_first; c0 < BN; c0 += c_step) {
             const int n0 = n_tile * BN + c0;
-            if (!row_ok || n0 >= p.N) continue;
+            if (n0 >= p.N) continue;
+            float v[32], g[32];
+            ld_row32(er, c0, v);
+            ld_row32(er, c0 + 32, g);
             T* o = reinterpret_cast<T*>(outp) + (n0 >> 1);
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -153,7 +135,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tmem
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     const int c = q * 8 + j;
-                    float a = __uint_as_float(v[c]) * p.alpha, b = __uint_as_float(g[c]) * p.alpha;
+                    float a = v[c] * p.alpha, b = g[c] * p.alpha;
                     if (bias) { a += Cvt<T>::to_f(bias[n0 + c]); b += Cvt<T>::to_f(bias[n0 + 32 + c]); }
                     h[j] = Cvt<T>::from_f(a * (0.5f * b * (1.0f + erff(b * 0.70710678118654752f))) * p.out_scale);
                 }
@@ -163,21 +145,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tmem
         return;
     }
 #pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t v[32];
-        ld_acc((uint32_t)c0, v);
-        tmem_ld_wait();
-        if (c0 + 32 >= BN) {
-            // accumulator fully read into registers: hand the TMEM buffer back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (REMOTE) mbar_arrive_cluster(release_bar); else mbar_arrive(release_bar); }
-        }
+    for (int c0 = c_first; c0 < BN; c0 += c_step) {
         const int n0 = n_tile * BN + c0;
-        if (!row_ok || n0 >= p.N) continue;
+        if (n0 >= p.N) continue;
         float f[32];
+        ld_row32(er, c0, f);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]) * p.alpha;
+        for (int j = 0; j < 32; ++j) f[j] *= p.alpha;
         const bool full = (n0 + 32 <= p.N);
         if (bias) {
 #pragma unroll
@@ -240,20 +214,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tmem
 }
 
 // CSD epilogue (dreammat_guidance.py:475-481 compute_grad_sds tail, :584 nan_to_num, the 8 logged norms of :483-495 and
-// loss_sds of :590-594) on the accumulator tile of branch k = 0 text | 1 uncond | 2 null.  The thread's row is pixel
+// loss_sds of :590-594) on the accumulator row of branch k = 0 text | 1 uncond | 2 null.  The thread's row is pixel
 // r = g*128 + row of the [view][pixel] axis; its 4 noise predictions (rounded to the storage dtype like the reference's
 // `.sample` in weights_dtype) wait in `e` until the third branch arrives, then
 //   grad = nan_to_num(w[b] * (c_t e_text + c_u e_uncond + c_n e_null + c_s noise)),  dlatents = grad * dlat_scale
 // are written (NCHW fp32) and the ten squared sums are reduced per warp and added to norms[10].
-template <int BN, typename T>
-__device__ __forceinline__ void epilogue_csd(const GemmParams& p, uint32_t tmem_acc, int64_t m, int lane, uint32_t release_bar,
-                                             float (&e)[2][4]) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(tmem_acc, v);
-    tmem_ld_wait();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(release_bar);
+template <typename T>
+__device__ __forceinline__ void epilogue_csd(const GemmParams& p, const float* er, int64_t m, int lane, float (&e)[2][4]) {
     const int64_t per_branch = (int64_t)p.csd_groups * BM;
     const int k = (int)(m / per_branch);
     const int64_t r = m - (int64_t)k * per_branch;
@@ -262,7 +229,7 @@ __device__ __forceinline__ void epilogue_csd(const GemmParams& p, uint32_t tmem_
     float cur[4];
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-        float f = __uint_as_float(v[c]);
+        float f = er[c];
         if (bias) f += Cvt<T>::to_f(bias[c]);
         cur[c] = Cvt<T>::to_f(Cvt<T>::from_f(f));
         if (p.csd_eps) p.csd_eps[(((int64_t)k * p.csd_B + b) * 4 + c) * p.csd_hw + px] = cur[c];
@@ -295,41 +262,32 @@ __device__ __forceinline__ void epilogue_csd(const GemmParams& p, uint32_t tmem_
     }
 }
 
-// CPS = persistent CTAs per SM.  Two co-resident CTAs (each with its own single-thread MMA issuer and a ~96 KB operand
-// ring) keep the tensor pipe's queue fuller for the narrower tiles; 256-wide tiles need all of TMEM and run one per SM.
-template <int BN, int CPS> struct Cfg {
+// ~128 KB operand ring + the fp32 staging tile of the epilogue (row pitch BN + 4 floats: conflict-free row reads).
+template <int BN> struct Cfg {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int RING = (CPS == 1) ? 196608 : 98304;
-    static constexpr int STAGES = RING / STAGE_BYTES;
-    static constexpr int ACC_STAGES = 2;                       // TMEM accumulator double buffer
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-    static constexpr int TMEM_COLS = (ACC_STAGES * BN) < 32 ? 32 : (ACC_STAGES * BN);
+    static constexpr int STAGES = 131072 / STAGE_BYTES;        // 4 (BN = 128) or 5 (BN = 64)
+    static constexpr int EPI_LD = BN + 4;
+    static constexpr int EPI_BYTES = BM * EPI_LD * 4;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
 
-// Persistent, warp-specialised kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...
-// The TMA producer runs ahead across tile boundaries, the MMA warp alternates between two TMEM accumulators and the
-// epilogue warps drain accumulator i while the tensor pipe already works on accumulator i^1.
-// DUAL = two accumulators per tile: even k-steps accumulate into one, odd k-steps into the other (two independent
-// dependency chains for the single issuing thread); the epilogue adds them.
-template <int BN, typename T, int CPS, bool DUAL = false>
-__global__ void __launch_bounds__(NTHREADS, CPS) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                              const __grid_constant__ CUtensorMap tmB,
-                                                              const GemmParams p) {
-    using C = Cfg<BN, CPS>;
-    constexpr int ACC_W = DUAL ? 2 * BN : BN;                                  // TMEM columns per accumulator stage
-    constexpr int TCOLS = (C::ACC_STAGES * ACC_W) < 32 ? 32 : (C::ACC_STAGES * ACC_W);
-    static_assert(TCOLS * CPS <= 512, "TMEM budget");
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES;
-    // barriers: full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], then the TMEM base address word
+// Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...
+template <int BN, typename T>
+__global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                             const __grid_constant__ CUtensorMap tmB,
+                                                             const GemmParams p) {
+    using C = Cfg<BN>;
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    const uint32_t raw_u32 = smem_u32(smem_raw);
+    const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;
+    float* epi = reinterpret_cast<float*>(smem_raw + (smem_base - raw_u32) + C::STAGES * C::STAGE_BYTES);
+    const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES + C::EPI_BYTES;
+    // barriers: full[STAGES] (TMA bytes landed), empty[STAGES] (both warpgroups done reading)
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-    auto tmem_full_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-    auto tmem_empty_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
 
     griddep_launch_dependents();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -342,18 +300,13 @@ __global__ void __launch_bounds__(NTHREADS, CPS) tc_gemm_kernel(const __grid_con
     if (threadIdx.x == 0) {
         prefetch_tmap(&tmA);
         prefetch_tmap(&tmB);
-        for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        for (int a = 0; a < C::ACC_STAGES; ++a) { mbar_init(tmem_full_bar(a), 1); mbar_init(tmem_empty_bar(a), 4); }
+        for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, TCOLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ld_shared_u32(tmem_slot);
     griddep_wait();      // PDL: everything above overlapped the previous kernel's tail; its outputs are visible from here
 
-    if (warp == 0) {
+    if (warp == CONSUMERS / 32) {
         if (lane == 0) {
             // ------------------------------------------------ TMA producer
             const int slabs = p.is_conv ? (p.Cin / BK) : nk;
@@ -388,372 +341,61 @@ __global__ void __launch_bounds__(NTHREADS, CPS) tc_gemm_kernel(const __grid_con
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ------------------------------------------------ MMA issuer (one thread)
-            constexpr uint32_t FMT = std::is_same<T, __half>::value ? 0u : 1u;
-            constexpr uint32_t IDESC = (1u << 4) | (FMT << 7) | (FMT << 10) | ((uint32_t)(BN >> 3) << 17) |
-                                       ((uint32_t)(BM >> 4) << 24);
-            int stage = 0; uint32_t phase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            for (int i = 0, t; (t = tile_at(p, i, blockIdx.x, gridDim.x, total_tiles)) >= 0; ++i) {
-                const int sp = t % S;
-                const int kb0 = (int)((int64_t)sp * nk / S), kb1 = (int)((int64_t)(sp + 1) * nk / S);
-                mbar_wait(tmem_empty_bar(acc), acc_phase ^ 1u);     // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * ACC_W);
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(full_bar(stage), phase);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_base + stage * C::STAGE_BYTES;
-                    const uint64_t da = make_sw128_desc(a_addr), db = make_sw128_desc(a_addr + C::A_BYTES);
+        return;
+    }
+    // -------------------------------------------------------- consumer warpgroups 0 / 1: MMA, then the epilogue
+    const int wg = warp >> 2;
+    const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // accumulator fragment rows frag_row, frag_row + 8
+    const int frag_col = 2 * (lane & 3);
+    const int ep_row = threadIdx.x & (BM - 1), ep_half = threadIdx.x >> 7;
+    int stage = 0; uint32_t phase = 0;
+    float csd_e[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+    float acc[BN / 2];
+    for (int i = 0, t; (t = tile_at(p, i, blockIdx.x, gridDim.x, total_tiles)) >= 0; ++i) {
+        const int sp = t % S, tt = t / S;
+        const int z = tt / tiles_per_z, r_ = tt - z * tiles_per_z;
+        const int m_tile = r_ / n_tiles, n_tile = r_ - m_tile * n_tiles;
+        const int kb0 = (int)((int64_t)sp * nk / S), kb1 = (int)((int64_t)(sp + 1) * nk / S);
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        // +32 bytes along K inside the 128-byte swizzle atom = +2 in the (addr >> 4) field
-                        umma_f16(tmem_d + ((DUAL && (k & 1)) ? (uint32_t)BN : 0u), da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), IDESC,
-                                 DUAL ? ((kb > kb0) || (k >= 2)) : (((kb - kb0) | k) != 0));
-                    }
-                    umma_commit(empty_bar(stage));
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-                }
-                umma_commit(tmem_full_bar(acc));
-                if (++acc == C::ACC_STAGES) { acc = 0; acc_phase ^= 1u; }
-            }
-        }
-    } else {
-        // ---------------------------------------------------- epilogue warps 2..5
-        const int quarter = warp & 3;           // TMEM lane quarter this warp may read
-        const int row = quarter * 32 + lane;    // row inside the tile
-        int acc = 0; uint32_t acc_phase = 0;
-        float csd_e[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-        for (int i = 0, t; (t = tile_at(p, i, blockIdx.x, gridDim.x, total_tiles)) >= 0; ++i) {
-            const int tt = t / S;
-            const int z = tt / tiles_per_z, r_ = tt - z * tiles_per_z;
-            const int m_tile = r_ / n_tiles, n_tile = r_ - m_tile * n_tiles;
-            const int64_t m = (int64_t)m_tile * BM + row;
-            mbar_wait(tmem_full_bar(acc), acc_phase);
-            tc_fence_after();
-            if constexpr (BN == 64 && !DUAL) {
-                if (p.csd) {
-                    epilogue_csd<BN, T>(p, tmem_base + (uint32_t)(acc * ACC_W) + ((uint32_t)(quarter * 32) << 16), m, lane,
-                                        tmem_empty_bar(acc), csd_e);
-                    if (++acc == C::ACC_STAGES) { acc = 0; acc_phase ^= 1u; }
-                    continue;
-                }
-            }
-            epilogue_tile<BN, T, false, DUAL>(p, tmem_base + (uint32_t)(acc * ACC_W) + ((uint32_t)(quarter * 32) << 16), m, z, n_tile,
-                                        lane, tmem_empty_bar(acc));
-            if (++acc == C::ACC_STAGES) { acc = 0; acc_phase ^= 1u; }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, TCOLS);
-}
-
-
-// ------------------------------------------------------------------------------------- CTA-pair kernel
-// cta_group::2: the two CTAs of a cluster (one TPC) compute one 256 x BN tile.  Each CTA stages its own 128 rows of A
-// and HALF of the BN weight rows; the leader's single MMA thread issues 256 x BN x 16 instructions that read A from
-// both CTAs' shared memory and the B halves from both, and write rows 0-127 / 128-255 of the accumulator into the
-// two CTAs' TMEM.  Per MMA each SM reads A (4 KB) + B/2 instead of A + B, which lifts the shared-memory-bandwidth
-// bound the single-CTA 128-wide tiles run into, and every weight tile is fetched from L2 once per 256 rows.
-// Barriers: full[s] lives in the leader (both CTAs' TMA loads credit their bytes to it), empty[s] / tmem_full[a]
-// are arrived on in BOTH CTAs by multicast tcgen05.commit, tmem_empty[a] in the leader collects the 8 epilogue warps.
-template <int BN> struct PairCfg {
-    static constexpr int A_BYTES = BM * BK * 2;
-    static constexpr int B_BYTES = (BN / 2) * BK * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = 196608 / STAGE_BYTES;        // 6 (BN = 256) or 8 (BN = 128)
-    static constexpr int ACC_STAGES = 2;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + 256;
-    static constexpr int ACC_STRIDE = BN <= 128 ? 128 : 256;   // TMEM columns between the two accumulators
-    static constexpr int TMEM_COLS = ACC_STAGES * ACC_STRIDE;  // power of two (BN = 160 rounds up)
-};
-
-template <int BN, typename T>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-    tc_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-    using C = PairCfg<BN>;
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES;
-    auto full_bar = [&](int s) { return bar_base + 8u * s; };
-    auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-    auto tmem_full_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-    auto tmem_empty_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-
-    griddep_launch_dependents();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const int nk = p.K / BK;
-    const int n_tiles = (p.N + BN - 1) / BN, m_pairs = (p.M + 2 * BM - 1) / (2 * BM);
-    const int tiles_per_z = n_tiles * m_pairs;
-    const int S = p.split_k > 1 ? p.split_k : 1;       // split-K over clusters, partial sums into p.ws
-    const int total_tiles = tiles_per_z * (p.batch > 0 ? p.batch : 1) * S;
-    const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-    if (threadIdx.x == 0) {
-        prefetch_tmap(&tmA);
-        prefetch_tmap(&tmB);
-        for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        for (int a = 0; a < C::ACC_STAGES; ++a) { mbar_init(tmem_full_bar(a), 1); mbar_init(tmem_empty_bar(a), 8); }
-        fence_mbar_init();
-    }
-    __syncwarp();
-    cluster_sync_all();                                  // both CTAs' barriers exist before any remote arrive
-    if (warp == 1) tmem_alloc_pair(tmem_slot, C::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ld_shared_u32(tmem_slot);
-    cluster_sync_all();                                  // the peer's TMEM is allocated before the first MMA lands in it
-    griddep_wait();                                      // PDL: the previous kernel's outputs are visible from here
-
-    if (warp == 0) {
-        if (lane == 0) {
-            // ------------------------------------------------ TMA producer (both CTAs)
-            const int slabs = p.is_conv ? (p.Cin / BK) : nk;
-            const int tiles_w = p.is_conv ? p.Wo / p.tile_w : 1, tiles_h = p.is_conv ? p.Ho / p.tile_h : 1;
-            int stage = 0; uint32_t phase = 0;
-            for (int t = cluster_id; t < total_tiles; t += n_clusters) {
-                const int sp = t % S, tt = t / S;
-                const int z = tt / tiles_per_z, r = tt - z * tiles_per_z;
-                const int m_tile = (r / n_tiles) * 2 + (int)rank, n_tile = r % n_tiles;
-                const int kb0 = (int)((int64_t)sp * nk / S), kb1 = (int)((int64_t)(sp + 1) * nk / S);
-                int c_n = 0, c_h = 0, c_w = 0;
-                if (p.is_conv) {
-                    int tw = m_tile % tiles_w, th = (m_tile / tiles_w) % tiles_h, tn = m_tile / (tiles_w * tiles_h);
-                    c_w = tw * p.tile_w * p.stride - p.pad_l;
-                    c_h = th * p.tile_h * p.stride - p.pad_t;
-                    c_n = tn * p.tile_n;                  // past the last image for a phantom tile: zero-filled
-                }
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(empty_bar(stage), phase ^ 1u);
-                    const uint32_t a_dst = smem_base + stage * C::STAGE_BYTES;
-                    const uint32_t b_dst = a_dst + C::A_BYTES;
-                    const uint32_t lead_full = full_bar(stage) & PAIR_LEADER_MASK;
-                    if (rank == 0) mbar_expect_tx(full_bar(stage), 2 * C::STAGE_BYTES);
-                    if (p.is_conv) {
-                        int tap = kb / slabs, slab = kb - tap * slabs;
-                        int kh = tap / p.kw_n, kw = tap - kh * p.kw_n;
-                        tma_load_4d_pair(a_dst, &tmA, lead_full, slab * BK, c_w + kw, c_h + kh, c_n);
-                    } else {
-                        tma_load_3d_pair(a_dst, &tmA, lead_full, kb * BK, m_tile * BM, z);
-                    }
-                    tma_load_3d_pair(b_dst, &tmB, lead_full, kb * BK, n_tile * BN + (int)rank * (BN / 2), p.b_batched ? z : 0);
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0 && lane == 0) {
-            // ------------------------------------------------ MMA issuer (one thread of the leader CTA)
-            constexpr uint32_t FMT = std::is_same<T, __half>::value ? 0u : 1u;
-            constexpr uint32_t IDESC = (1u << 4) | (FMT << 7) | (FMT << 10) | ((uint32_t)(BN >> 3) << 17) |
-                                       ((uint32_t)((2 * BM) >> 4) << 24);
-            int stage = 0; uint32_t phase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            for (int t = cluster_id; t < total_tiles; t += n_clusters) {
-                const int sp = t % S;
-                const int kb0 = (int)((int64_t)sp * nk / S), kb1 = (int)((int64_t)(sp + 1) * nk / S);
-                mbar_wait(tmem_empty_bar(acc), acc_phase ^ 1u);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * C::ACC_STRIDE);
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(full_bar(stage), phase);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_base + stage * C::STAGE_BYTES;
-                    const uint64_t da = make_sw128_desc(a_addr), db = make_sw128_desc(a_addr + C::A_BYTES);
+        for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(full_bar(stage), phase);
+            const uint32_t a_addr = smem_base + stage * C::STAGE_BYTES;
+            const uint64_t da = make_sw128_desc(a_addr + (uint32_t)wg * (64 * 128)), db = make_sw128_desc(a_addr + C::A_BYTES);
+            wgmma_fence();
+            wgmma_fence_operands(acc);
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k)
-                        umma_f16_pair(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), IDESC, ((kb - kb0) | k) != 0);
-                    umma_commit_pair(empty_bar(stage), 3);
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-                }
-                umma_commit_pair(tmem_full_bar(acc), 3);
-                if (++acc == C::ACC_STAGES) { acc = 0; acc_phase ^= 1u; }
-            }
+            for (int k = 0; k < BK / 16; ++k) Wgmma<BN, T>::ss(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k));
+            wgmma_commit();
+            wgmma_fence_operands(acc);
+            wgmma_wait<1>();                       // the previous k-block's MMAs are done: hand its stage back
+            if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev));
+            prev = stage;
+            if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
         }
-    } else {
-        // ---------------------------------------------------- epilogue warps 2..5 (both CTAs, own 128 rows)
-        const int quarter = warp & 3;
-        const int row = quarter * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int t = cluster_id; t < total_tiles; t += n_clusters) {
-            const int tt = t / S;
-            const int z = tt / tiles_per_z, r_ = tt - z * tiles_per_z;
-            const int m_tile = (r_ / n_tiles) * 2 + (int)rank, n_tile = r_ % n_tiles;
-            const int64_t m = (int64_t)m_tile * BM + row;
-            mbar_wait(tmem_full_bar(acc), acc_phase);
-            tc_fence_after();
-            epilogue_tile<BN, T, true>(p, tmem_base + (uint32_t)(acc * C::ACC_STRIDE) + ((uint32_t)(quarter * 32) << 16), m, z, n_tile,
-                                       lane, tmem_empty_bar(acc) & PAIR_LEADER_MASK);
-            if (++acc == C::ACC_STAGES) { acc = 0; acc_phase ^= 1u; }
-        }
-    }
-    __syncwarp();
-    tc_fence_before();
-    cluster_sync_all();          // nobody leaves (or frees TMEM) while the other CTA may still signal / be written
-    if (warp == 1) tmem_dealloc_pair(tmem_base, C::TMEM_COLS);
-}
-
-
-// ------------------------------------------------------------------------------------- halo-reuse 3x3 convolution (CTA pair)
-// EXPERIMENT, off by default (dm_tune_gemm 31 / 32).  For stride-1 3x3 convolutions whose output rows are >= 128 pixels
-// wide (the VAE's 512^2 / 256^2 / 128^2 levels) a 128-pixel M tile is one image-row segment, so the nine taps' A operands
-// are nine SHIFTED windows of one (3 rows x 130 pixels x 64 channels) halo tile: window (kh, kw) = 128 consecutive
-// 128-byte rows starting at row kh * 130 + kw of the halo.  The halo is fetched ONCE per 64-channel slab (one 4-D TMA
-// box, out-of-bounds rows / columns zero-filled = padding) instead of nine 16 KB tiles, and the UMMA descriptor's start
-// address is simply advanced by (kh * 130 + kw) * 128 bytes.  Per CTA and slab: 50 KB halo + 9 weight half-tiles instead of
-// 144 KB + 9 -- the N = 128 layers (operand-traffic bound at ~1.0 PFLOP/s today) drop from 96 to ~53 B/clk/SM.
-// HALO_MODE 1: descriptor base_offset = (start >> 7) & 7 (the 128B-swizzle phase of a start that is not 1024-byte aligned);
-// HALO_MODE 2: base_offset left 0 (if the hardware derives the phase from the address bits themselves).
-constexpr int HALO_W = 130, HALO_ROWS = 3 * HALO_W;
-constexpr int HALO_TX = HALO_ROWS * 128;                         // bytes one halo TMA delivers (49 920)
-constexpr int HALO_BYTES = (HALO_TX + 1023) / 1024 * 1024;       // stage size, keeps 1024-byte alignment (51 200)
-template <int BN> struct HaloCfg {
-    static constexpr int HS = 2;                                 // halo stages
-    static constexpr int B_BYTES = (BN / 2) * BK * 2;
-    static constexpr int BS = BN == 256 ? 6 : 8;                 // weight half-tile stages
-    static constexpr int ACC_STAGES = 2;
-    static constexpr int SMEM = HS * HALO_BYTES + BS * B_BYTES + 1024 + 256;
-    static constexpr int TMEM_COLS = ACC_STAGES * BN;
-};
-
-template <int BN, typename T, int HALO_MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-    tc_conv_halo_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-    using C = HaloCfg<BN>;
-    extern __shared__ uint8_t smem_raw[];
-    griddep_launch_dependents();
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t b_base = smem_base + C::HS * HALO_BYTES;
-    const uint32_t bar_base = b_base + C::BS * C::B_BYTES;
-    auto full_h = [&](int s) { return bar_base + 8u * s; };
-    auto empty_h = [&](int s) { return bar_base + 8u * (C::HS + s); };
-    auto full_b = [&](int s) { return bar_base + 8u * (2 * C::HS + s); };
-    auto empty_b = [&](int s) { return bar_base + 8u * (2 * C::HS + C::BS + s); };
-    auto tmem_full_bar = [&](int a) { return bar_base + 8u * (2 * C::HS + 2 * C::BS + a); };
-    auto tmem_empty_bar = [&](int a) { return bar_base + 8u * (2 * C::HS + 2 * C::BS + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * C::HS + 2 * C::BS + 4);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const int slabs = p.Cin / BK;
-    const int n_tiles = (p.N + BN - 1) / BN, m_pairs = (p.M + 2 * BM - 1) / (2 * BM);
-    const int total_tiles = n_tiles * m_pairs;
-    const int tiles_w = p.Wo / BM;
-    const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-    if (threadIdx.x == 0) {
-        prefetch_tmap(&tmH);
-        prefetch_tmap(&tmB);
-        for (int s = 0; s < C::HS; ++s) { mbar_init(full_h(s), 1); mbar_init(empty_h(s), 1); }
-        for (int s = 0; s < C::BS; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), 1); }
-        for (int a = 0; a < C::ACC_STAGES; ++a) { mbar_init(tmem_full_bar(a), 1); mbar_init(tmem_empty_bar(a), 8); }
-        fence_mbar_init();
-    }
-    __syncwarp();
-    cluster_sync_all();
-    if (warp == 1) tmem_alloc_pair(tmem_slot, C::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ld_shared_u32(tmem_slot);
-    cluster_sync_all();
-    griddep_wait();
-
-    if (warp == 0) {
-        if (lane == 0) {
-            // ------------------------------------------------ TMA producer (both CTAs): halo(s+1) is requested before the nine
-            // weight tiles of slab s, so it lands while slab s is still being multiplied
-            int hs = 0; uint32_t hphase = 0; int bs = 0; uint32_t bphase = 0;
-            auto issue_halo = [&](int t, int slab) {
-                const int r = t;                                   // batch == 1
-                const int m_tile = (r / n_tiles) * 2 + (int)rank;
-                const int tw = m_tile % tiles_w, th = (m_tile / tiles_w) % p.Ho, tn = m_tile / (tiles_w * p.Ho);
-                mbar_wait(empty_h(hs), hphase ^ 1u);
-                if (rank == 0) mbar_expect_tx(full_h(hs), 2 * HALO_TX);
-                tma_load_4d_pair(smem_base + hs * HALO_BYTES, &tmH, full_h(hs) & PAIR_LEADER_MASK, slab * BK, tw * BM - 1, th - 1, tn);
-                if (++hs == C::HS) { hs = 0; hphase ^= 1u; }
-            };
-            // flattened stream of (tile, slab) pairs
-            int t = cluster_id, slab = 0;
-            bool have = t < total_tiles;
-            if (have) issue_halo(t, 0);
-            while (have) {
-                int nt = t, nslab = slab + 1;
-                if (nslab == slabs) { nslab = 0; nt = t + n_clusters; }
-                const bool have_next = nt < total_tiles;
-                if (have_next) issue_halo(nt, nslab);
-                const int n_tile = t % n_tiles;
-                for (int tap = 0; tap < 9; ++tap) {
-                    mbar_wait(empty_b(bs), bphase ^ 1u);
-                    if (rank == 0) mbar_expect_tx(full_b(bs), 2 * C::B_BYTES);
-                    tma_load_3d_pair(b_base + bs * C::B_BYTES, &tmB, full_b(bs) & PAIR_LEADER_MASK, (tap * slabs + slab) * BK,
-                                     n_tile * BN + (int)rank * (BN / 2), 0);
-                    if (++bs == C::BS) { bs = 0; bphase ^= 1u; }
-                }
-                t = nt; slab = nslab; have = have_next;
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0 && lane == 0) {
-            // ------------------------------------------------ MMA issuer (leader CTA)
-            constexpr uint32_t FMT = std::is_same<T, __half>::value ? 0u : 1u;
-            constexpr uint32_t IDESC = (1u << 4) | (FMT << 7) | (FMT << 10) | ((uint32_t)(BN >> 3) << 17) |
-                                       ((uint32_t)((2 * BM) >> 4) << 24);
-            int hs = 0; uint32_t hphase = 0; int bs = 0; uint32_t bphase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            for (int t = cluster_id; t < total_tiles; t += n_clusters) {
-                mbar_wait(tmem_empty_bar(acc), acc_phase ^ 1u);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-                for (int slab = 0; slab < slabs; ++slab) {
-                    mbar_wait(full_h(hs), hphase);
-                    tc_fence_after();
-                    const uint32_t h_addr = smem_base + hs * HALO_BYTES;
-                    for (int tap = 0; tap < 9; ++tap) {
-                        mbar_wait(full_b(bs), bphase);
-                        tc_fence_after();
-                        const int kh = tap / 3, kw = tap - kh * 3;
-                        const uint32_t a_addr = h_addr + (uint32_t)((kh * HALO_W + kw) * 128);
-                        uint64_t da = make_sw128_desc(a_addr);
-                        if (HALO_MODE == 1) da |= (uint64_t)((a_addr >> 7) & 7u) << 49;     // swizzle phase of the shifted start
-                        const uint64_t db = make_sw128_desc(b_base + bs * C::B_BYTES);
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev));
+        named_bar_sync(1, CONSUMERS);              // the previous tile's epilogue has finished reading the staging tile
 #pragma unroll
-                        for (int k = 0; k < BK / 16; ++k)
-                            umma_f16_pair(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), IDESC, (slab | tap | k) != 0);
-                        umma_commit_pair(empty_b(bs), 3);
-                        if (++bs == C::BS) { bs = 0; bphase ^= 1u; }
-                    }
-                    umma_commit_pair(empty_h(hs), 3);
-                    if (++hs == C::HS) { hs = 0; hphase ^= 1u; }
-                }
-                umma_commit_pair(tmem_full_bar(acc), 3);
-                if (++acc == C::ACC_STAGES) { acc = 0; acc_phase ^= 1u; }
+        for (int j = 0; j < BN / 8; ++j) {
+            *reinterpret_cast<float2*>(epi + frag_row * C::EPI_LD + 8 * j + frag_col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(epi + (frag_row + 8) * C::EPI_LD + 8 * j + frag_col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        named_bar_sync(1, CONSUMERS);
+        const int64_t m = (int64_t)m_tile * BM + ep_row;
+        const float* er = epi + ep_row * C::EPI_LD;
+        if constexpr (BN == 64) {
+            if (p.csd) {
+                if (ep_half == 0) epilogue_csd<T>(p, er, m, lane, csd_e);
+                continue;
             }
         }
-    } else {
-        const int quarter = warp & 3;
-        const int row = quarter * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int t = cluster_id; t < total_tiles; t += n_clusters) {
-            const int m_tile = (t / n_tiles) * 2 + (int)rank, n_tile = t % n_tiles;
-            const int64_t m = (int64_t)m_tile * BM + row;
-            mbar_wait(tmem_full_bar(acc), acc_phase);
-            tc_fence_after();
-            epilogue_tile<BN, T, true>(p, tmem_base + (uint32_t)(acc * BN) + ((uint32_t)(quarter * 32) << 16), m, 0, n_tile, lane,
-                                       tmem_empty_bar(acc) & PAIR_LEADER_MASK);
-            if (++acc == C::ACC_STAGES) { acc = 0; acc_phase ^= 1u; }
-        }
+        // the two threads of a row split its column chunks (GEGLU chunks are 64 wide)
+        const int step = p.act == 3 ? 64 : 32;
+        epilogue_row<BN, T>(p, er, m, z, sp, n_tile, ep_half * step, 2 * step);
     }
-    __syncwarp();
-    tc_fence_before();
-    cluster_sync_all();
-    if (warp == 1) tmem_dealloc_pair(tmem_base, C::TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------- host side
@@ -794,53 +436,30 @@ int encode_map(CUtensorMap* m, int bf16, const void* base, int rank, const uint6
     return DM_OK;
 }
 
-int g_gemm_cps = 2;   // persistent CTAs per SM for BN <= 128 (dm_tune "gemm_cps")
-
-int g_gemm_dual = 0;   // two accumulators per tile in the single-CTA kernel for BN <= 128 (dm_tune_gemm 40 / 41)
-
-template <int BN, typename T, int CPS, bool DUAL = false>
-int launch_cps(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
+template <int BN, typename T>
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int64_t work_items, cudaStream_t st) {
     static bool configured = false;
-    auto kern = tc_gemm_kernel<BN, T, CPS, DUAL>;
+    auto kern = tc_gemm_kernel<BN, T>;
     if (!configured) {
-        DM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN, CPS>::SMEM));
+        DM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM));
         configured = true;
     }
-    int64_t tiles = dm_ceil_div(p.N, BN) * dm_ceil_div(p.M, BM) * (p.batch > 0 ? p.batch : 1) * (p.split_k > 1 ? p.split_k : 1);
-    int64_t slots = (int64_t)DM_NUM_SMS * CPS;
-    unsigned grid = (unsigned)(tiles < slots ? tiles : slots);   // persistent: CPS CTAs per SM
-    DM_CHECK_CUDA(dm_launch(kern, dim3(grid), dim3(NTHREADS), (size_t)Cfg<BN, CPS>::SMEM, st, tmA, tmB, p));
+    unsigned grid = (unsigned)(work_items < DM_NUM_SMS ? work_items : DM_NUM_SMS);   // persistent: one CTA per SM
+    DM_CHECK_CUDA(dm_launch(kern, dim3(grid), dim3(NTHREADS), (size_t)Cfg<BN>::SMEM, st, tmA, tmB, p));
     DM_CHECK_LAUNCH();
     return DM_OK;
 }
 
-template <int BN, typename T>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
-    if constexpr (BN <= 128) {
-        // two co-resident CTAs only pay when there are more tiles than SMs; otherwise one CTA per SM with the full
-        // 192 KB ring (twice the loads in flight) hides the L2/HBM latency of the long-K, few-tile layers better
-        int64_t tiles = dm_ceil_div(p.N, BN) * dm_ceil_div(p.M, BM) * (p.batch > 0 ? p.batch : 1) * (p.split_k > 1 ? p.split_k : 1);
-        const bool two = g_gemm_cps == 2 && tiles > DM_NUM_SMS;
-        if (g_gemm_dual && p.act != 3) {
-            if constexpr (BN == 64) { if (two) return launch_cps<BN, T, 2, true>(tmA, tmB, p, st); }
-            return launch_cps<BN, T, 1, true>(tmA, tmB, p, st);      // 128-wide dual needs all 512 TMEM columns
-        }
-        if (two) return launch_cps<BN, T, 2>(tmA, tmB, p, st);
-    }
-    return launch_cps<BN, T, 1>(tmA, tmB, p, st);
-}
-
 // ---- split-K: few-tile, long-K layers (8x8 / 16x16 latents of a one-view batch) leave most SMs idle; S CTAs share a tile,
-// red.add fp32 partials into a zeroed workspace, and this kernel applies the epilogue and re-zeroes the workspace.
+// each stores its fp32 partial tile in its own workspace slice, and this kernel adds the S slices in order and applies the
+// epilogue.
 float* g_ws = nullptr;
 size_t g_ws_floats = 0;
 int g_gemm_splitk = 1;
-constexpr size_t WS_FLOATS = 8u << 20;   // recommended size, 32 MB: M*N <= 8 M elements (dm_gemm_workspace_bytes)
+constexpr size_t WS_FLOATS = 8u << 20;   // recommended size, 32 MB: S*M*N <= 8 M elements (dm_gemm_workspace_bytes)
 
 // The workspace is owned by the caller (dm_gemm_set_workspace): no hidden allocation inside the library.  Without one,
 // split-K is simply not used.
-bool ensure_ws(size_t floats, cudaStream_t) { return g_ws != nullptr && floats <= g_ws_floats; }
-
 template <typename T>
 __global__ void __launch_bounds__(256) splitk_finish_kernel(const GemmParams p) {
     griddep_launch_dependents();
@@ -851,9 +470,12 @@ __global__ void __launch_bounds__(256) splitk_finish_kernel(const GemmParams p) 
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t row = i / n4; const int c = (int)(i - row * n4) * 4;
         const int z = (int)(row / p.M); const int64_t m = row - (int64_t)z * p.M;
-        float4* w4 = reinterpret_cast<float4*>(p.ws + row * p.N + c);
-        float4 a = *w4;
-        *w4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int64_t slice = total * 4;
+        float4 a = *reinterpret_cast<const float4*>(p.ws + row * p.N + c);
+        for (int sp = 1; sp < p.split_k; ++sp) {
+            const float4 b = *reinterpret_cast<const float4*>(p.ws + sp * slice + row * p.N + c);
+            a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        }
         float f[4] = {a.x * p.alpha, a.y * p.alpha, a.z * p.alpha, a.w * p.alpha};
         if (bias) {
 #pragma unroll
@@ -887,141 +509,57 @@ __global__ void __launch_bounds__(256) splitk_finish_kernel(const GemmParams p) 
     }
 }
 
-// split factor for a single-CTA launch of `tiles` output tiles with nk K-blocks (1 = no split)
-int pick_split(int64_t tiles, int nk, int64_t mn, int N, int act, bool out_ok, cudaStream_t st) {
-    if (!g_gemm_splitk || act == 3 || (N & 3) || !out_ok) return 1;
+struct TileChoice { int bn; int split; };   // split: 0 = let dispatch decide, >= 1 fixed
+
+// Tile width: 64 when there are fewer 128 x 128 tiles than SMs (low-resolution UNet levels) or N <= 64, else 128.  The
+// 128 x 128 tile keeps both warpgroups' m64n128 accumulators (64 fp32 registers per thread) and a four-stage operand ring
+// in one SM; a 256-wide tile would not leave room for the epilogue's staging tile, so a 256 hint gets 128.
+int pick_bn(int64_t M, int N, int bn_hint) {
+    if (bn_hint == 64) return 64;
+    if (bn_hint == 128 || bn_hint == 256) return 128;
+    if (N <= 64) return 64;
+    int64_t tiles128 = dm_ceil_div(M, BM) * dm_ceil_div(N, 128);
+    if (tiles128 < (int64_t)DM_NUM_SMS && N % 64 == 0) return 64;
+    return 128;
+}
+
+// split factor for `tiles` output tiles with nk K-blocks (1 = no split): only when at most half the SMs would have a
+// tile and the K loop is long enough to amortise the workspace pass.  The split also keeps each CTA's accumulation chain
+// near 64 K-blocks: the wgmma fp32 accumulator drifts over longer chains (fp32-mode error vs fp64 measured on the
+// H100: 4.4e-6 at 60 blocks, 1.5e-5 at 160, 2.1e-5 at 360), which the 6x-long K of the fp32 mode would otherwise hit.
+int pick_split(int64_t tiles, int nk, int64_t mn, int N, int act) {
+    if (!g_gemm_splitk || act == 3 || (N & 3)) return 1;
     if (tiles * 2 > DM_NUM_SMS || nk < 32) return 1;
     int s = (int)(DM_NUM_SMS / tiles);
+    if (s < (nk + 63) / 64) s = (nk + 63) / 64;
     if (s > nk / 8) s = nk / 8;
     if (s > 16) s = 16;
-    if (s < 2 || !ensure_ws((size_t)mn, st)) return 1;
+    if (g_ws != nullptr && (size_t)mn * s > g_ws_floats) s = (int)(g_ws_floats / (size_t)mn);   // one workspace slice per split
+    if (s < 2 || g_ws == nullptr) return 1;
     return s;
 }
 
-int g_gemm_pair = 1;  // 0 never, 1 where measured faster (use_pair), 2 wherever the shape allows (dm_tune_gemm 10/11/12)
-
-template <int BN, typename T>
-int launch_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
-    static int max_clusters = 0;
-    auto kern = tc_gemm_pair_kernel<BN, T>;
-    if (!max_clusters) {
-        DM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PairCfg<BN>::SMEM));
-        cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(DM_NUM_SMS); cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = PairCfg<BN>::SMEM;
-        cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
-        cfg.attrs = &at; cfg.numAttrs = 1;
-        int n = 0;
-        if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n < 1) { cudaGetLastError(); n = DM_NUM_SMS / 2; }
-        max_clusters = n < DM_NUM_SMS / 2 ? n : DM_NUM_SMS / 2;
-    }
-    int64_t tiles = dm_ceil_div(p.N, BN) * dm_ceil_div(p.M, 2 * BM) * (p.batch > 0 ? p.batch : 1) * (p.split_k > 1 ? p.split_k : 1);
-    unsigned clusters = (unsigned)(tiles < max_clusters ? tiles : max_clusters);
-    DM_CHECK_CUDA(dm_launch(kern, dim3(2 * clusters), dim3(NTHREADS), (size_t)PairCfg<BN>::SMEM, st, tmA, tmB, p));
-    DM_CHECK_LAUNCH();
-    return DM_OK;
-}
-
-struct TileChoice { int bn; bool pair; int split; };   // split: 0 = let dispatch decide (single-CTA path), >= 1 fixed
-
-int pick_bn(int64_t M, int N, int bn_hint);
-
-// Tile width and single-CTA vs CTA-pair kernel.  bn_hint: 0 auto; 64/128/256 single-CTA kernel of that width;
-// 1000 + {128,160,256} CTA-pair kernel of that width (experiments / tests).
-TileChoice choose_tile(int64_t M, int N, int nk, int bn_hint, int act) {
-    if (bn_hint >= 1000) return {bn_hint - 1000, true, 1};
-    if (bn_hint == 64 || bn_hint == 128 || bn_hint == 256) return {bn_hint, g_gemm_pair == 2 && bn_hint >= 128, g_gemm_pair == 2 && bn_hint >= 128 ? 1 : 0};
-    if (g_gemm_pair) {
-        // wide pair tiles: every SM reads A + B/2 per MMA and each weight tile is fetched once per 256 rows.  Measured
-        // (scripts/sweep_tiles.py, profiles/r01_tile_sweep.md): 256-wide pairs beat the best single-CTA tile by 1.1-1.4x
-        // once there are >= 74 pair tiles (also for N = 640 / 960 / 1920 despite the padded last tile); 160-wide pairs
-        // (N = 320: two exact tiles) win by ~7 % but only with several waves of tiles.
-        const int64_t mp = dm_ceil_div(M, 2 * BM);
-        const int64_t tpcs = DM_NUM_SMS / 2;
-        if (N >= 512 || N == 256) {
-            const int64_t pt = mp * dm_ceil_div(N, 256);
-            if (pt >= tpcs) return {256, true, 1};
-            // few tiles: the layer is bound by L2->SMEM bytes (~12 TB/s chip-wide), which wide pair tiles cut 2-3x
-            // against 64-wide tiles; split-K spreads the K loop over the idle TPCs
-            // (the workspace pass costs ~10 us: only long K loops amortise it -- measured in scripts/exp_splitk.py)
-            if (g_gemm_splitk && act != 3 && (N & 3) == 0 && (nk >= 128 || (nk >= 64 && pt <= 8)) && g_ws != nullptr && (size_t)(M * N) <= g_ws_floats) {
-                int64_t sp = tpcs / pt;
-                if (sp > nk / 8) sp = nk / 8;
-                if (sp > 16) sp = 16;
-                if (sp >= 2) return {256, true, (int)sp};
-            }
-            if (2 * pt >= tpcs) return {256, true, 1};
-        } else if (N % 160 == 0 && act != 3) {
-            if (mp * (N / 160) >= 3 * tpcs) return {160, true, 1};
-        }
-    }
-    return {pick_bn(M, N, 0), false, 0};
-}
-
-int dispatch_single(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int bn, int bf16, cudaStream_t st);
-
-int dispatch_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int bn, int bf16, cudaStream_t st) {
-    if (bf16) {
-        if (bn == 128) return launch_pair<128, __nv_bfloat16>(tmA, tmB, p, st);
-        if (bn == 160) return launch_pair<160, __nv_bfloat16>(tmA, tmB, p, st);
-        if (bn == 256) return launch_pair<256, __nv_bfloat16>(tmA, tmB, p, st);
-    } else {
-        if (bn == 128) return launch_pair<128, __half>(tmA, tmB, p, st);
-        if (bn == 160) return launch_pair<160, __half>(tmA, tmB, p, st);
-        if (bn == 256) return launch_pair<256, __half>(tmA, tmB, p, st);
-    }
-    dm_set_error("unsupported pair tile width %d", bn);
-    return DM_EUNSUPPORTED;
-}
+TileChoice choose_tile(int64_t M, int N, int bn_hint) { return {pick_bn(M, N, bn_hint), 0}; }
 
 int dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p_in, const TileChoice& tc, int bf16, cudaStream_t st) {
     GemmParams p = p_in;
     const int64_t batch = p.batch > 0 ? p.batch : 1;
-    int split = 1;
-    if (tc.pair) {
-        if (tc.split > 1 && ensure_ws((size_t)(batch * p.M * p.N), st)) split = tc.split;
-    } else {
-        const int64_t tiles = dm_ceil_div(p.N, tc.bn) * dm_ceil_div(p.M, BM) * batch;
-        split = tc.split >= 1 ? 1 : pick_split(tiles, p.K / BK, batch * p.M * p.N, p.N, p.act, true, st);
-    }
+    const int64_t tiles = dm_ceil_div(p.N, tc.bn) * dm_ceil_div(p.M, BM) * batch;
+    const int split = tc.split >= 1 ? tc.split : pick_split(tiles, p.K / BK, batch * p.M * p.N, p.N, p.act);
     p.split_k = split;
     p.ws = split > 1 ? g_ws : nullptr;
-    int rc = tc.pair ? dispatch_pair(tmA, tmB, p, tc.bn, bf16, st) : dispatch_single(tmA, tmB, p, tc.bn, bf16, st);
+    const int64_t work = tiles * split;
+    int rc;
+    if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, p, work, st) : launch<64, __half>(tmA, tmB, p, work, st);
+    else rc = bf16 ? launch<128, __nv_bfloat16>(tmA, tmB, p, work, st) : launch<128, __half>(tmA, tmB, p, work, st);
     if (rc || split <= 1) return rc;
-    const int64_t work = batch * p.M * (p.N >> 2);
-    int64_t blocks = dm_ceil_div(work, 256);
+    const int64_t n4 = batch * p.M * (p.N >> 2);
+    int64_t blocks = dm_ceil_div(n4, 256);
     if (blocks > DM_NUM_SMS * 8) blocks = DM_NUM_SMS * 8;
     if (bf16) DM_CHECK_CUDA(dm_launch(splitk_finish_kernel<__nv_bfloat16>, dim3((unsigned)blocks), dim3(256), 0, st, p));
     else DM_CHECK_CUDA(dm_launch(splitk_finish_kernel<__half>, dim3((unsigned)blocks), dim3(256), 0, st, p));
     DM_CHECK_LAUNCH();
     return DM_OK;
-}
-
-int dispatch_single(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int bn, int bf16, cudaStream_t st) {
-    if (bf16) {
-        if (bn == 64) return launch<64, __nv_bfloat16>(tmA, tmB, p, st);
-        if (bn == 128) return launch<128, __nv_bfloat16>(tmA, tmB, p, st);
-        if (bn == 256) return launch<256, __nv_bfloat16>(tmA, tmB, p, st);
-    } else {
-        if (bn == 64) return launch<64, __half>(tmA, tmB, p, st);
-        if (bn == 128) return launch<128, __half>(tmA, tmB, p, st);
-        if (bn == 256) return launch<256, __half>(tmA, tmB, p, st);
-    }
-    dm_set_error("unsupported BN %d", bn);
-    return DM_EUNSUPPORTED;
-}
-
-int pick_bn(int64_t M, int N, int bn_hint) {
-    if (bn_hint == 64 || bn_hint == 128 || bn_hint == 256) return bn_hint;
-    if (N <= 64) return 64;
-    // fewer 128x128 tiles than SMs: halve the tile width so every SM gets work (low-resolution UNet levels)
-    int64_t tiles128 = dm_ceil_div(M, BM) * dm_ceil_div(N, 128);
-    if (tiles128 < (int64_t)DM_NUM_SMS && N % 64 == 0) return 64;
-    // wide tiles (one 128x256x16 MMA = 128 tensor-pipe cycles per issue) feed the single issuing thread of the
-    // persistent CTA best: measured 1384 vs 1173 TFLOP/s on 8192x4096x4096
-    if (N % 256 == 0 && dm_ceil_div(M, BM) * (N / 256) >= (int64_t)DM_NUM_SMS) return 256;
-    // 128-wide tiles even when N is not a multiple (320 -> 3 tiles, 17 % padding): measured 783 vs 653 TFLOP/s
-    // against 64-wide tiles on the 320-channel convolutions
-    return 128;
 }
 
 void fill_epilogue(GemmParams& p, const dm_epilogue* e, int N) {
@@ -1038,53 +576,17 @@ void fill_epilogue(GemmParams& p, const dm_epilogue* e, int N) {
     p.out_f32 = e ? e->out_f32 : 0;
 }
 
-
-int g_gemm_halo = 0;   // 0 off, 1 / 2 = HALO_MODE of tc_conv_halo_kernel (dm_tune_gemm 30 / 31 / 32)
-
-template <int BN, typename T, int MODE>
-int launch_halo(const CUtensorMap& tmH, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
-    static bool configured = false;
-    auto kern = tc_conv_halo_kernel<BN, T, MODE>;
-    if (!configured) {
-        DM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, HaloCfg<BN>::SMEM));
-        configured = true;
-    }
-    int64_t tiles = dm_ceil_div(p.N, BN) * dm_ceil_div(p.M, 2 * BM);
-    unsigned clusters = (unsigned)(tiles < DM_NUM_SMS / 2 ? tiles : DM_NUM_SMS / 2);
-    DM_CHECK_CUDA(dm_launch(kern, dim3(2 * clusters), dim3(NTHREADS), (size_t)HaloCfg<BN>::SMEM, st, tmH, tmB, p));
-    DM_CHECK_LAUNCH();
-    return DM_OK;
-}
-
-template <int BN>
-int dispatch_halo(const CUtensorMap& tmH, const CUtensorMap& tmB, const GemmParams& p, int bf16, cudaStream_t st) {
-    if (g_gemm_halo == 2) return bf16 ? launch_halo<BN, __nv_bfloat16, 2>(tmH, tmB, p, st) : launch_halo<BN, __half, 2>(tmH, tmB, p, st);
-    return bf16 ? launch_halo<BN, __nv_bfloat16, 1>(tmH, tmB, p, st) : launch_halo<BN, __half, 1>(tmH, tmB, p, st);
-}
-
 }  // namespace
 
 // Pure query of the tile heuristic (no launch): which kernel / tile width / split-K a [M, N, K] contraction would get.
-// kernel_out: 0 single-CTA, 1 CTA pair.  split_out is the pair path's request, or for the single-CTA path what
-// pick_split would choose given a registered workspace.  Lets host-side tests pin the measured choices.
+// kernel_out is always 0 (one single-CTA kernel); split_out is what pick_split would choose given the registered
+// workspace.  Lets host-side tests pin the choices.
 extern "C" int dm_gemm_plan(int64_t M, int N, int K, int act, int bn_hint, int* kernel_out, int* bn_out, int* split_out) {
     DM_REQUIRE(M > 0 && N > 0 && K > 0 && K % BK == 0 && kernel_out && bn_out && split_out, "bad args");
-    TileChoice tc = choose_tile(M, N, K / BK, bn_hint, act);
-    *kernel_out = tc.pair ? 1 : 0;
+    TileChoice tc = choose_tile(M, N, bn_hint);
+    *kernel_out = 0;
     *bn_out = tc.bn;
-    int split = tc.split > 1 ? tc.split : 1;
-    if (!tc.pair && tc.split == 0) {
-        const int64_t tiles = dm_ceil_div(N, tc.bn) * dm_ceil_div(M, BM);
-        const int nk = K / BK;
-        if (g_gemm_splitk && act != 3 && (N & 3) == 0 && tiles * 2 <= DM_NUM_SMS && nk >= 32 && g_ws != nullptr &&
-            (size_t)(M * N) <= g_ws_floats) {
-            int s2 = (int)(DM_NUM_SMS / tiles);
-            if (s2 > nk / 8) s2 = nk / 8;
-            if (s2 > 16) s2 = 16;
-            if (s2 >= 2) split = s2;
-        }
-    }
-    *split_out = split;
+    *split_out = pick_split(dm_ceil_div(N, tc.bn) * dm_ceil_div(M, BM), K / BK, M * N, N, act);
     return DM_OK;
 }
 
@@ -1097,12 +599,9 @@ extern "C" int dm_gemm_set_workspace(void* ptr, size_t bytes) {
 }
 
 extern "C" int dm_tune_gemm(int code) {
-    if (code >= 10 && code <= 12) g_gemm_pair = code - 10;      // CTA-pair kernel: 10 off, 11 heuristic, 12 always
-    else if (code == 20 || code == 21) g_gemm_splitk = code - 20;  // split-K of few-tile long-K layers: off | on
-    else if (code == 40 || code == 41) g_gemm_dual = code - 40;    // two accumulators per tile (single-CTA kernel, BN <= 128): off | on
-    else if (code >= 30 && code <= 32) g_gemm_halo = code - 30;    // halo-reuse 3x3 conv experiment: off | mode 1 | mode 2
-    else g_gemm_cps = code == 1 ? 1 : 2;                        // single-CTA kernel: persistent CTAs per SM
-    return DM_OK;
+    if (code == 20 || code == 21) { g_gemm_splitk = code - 20; return DM_OK; }   // split-K of few-tile long-K layers: off | on
+    dm_set_error("dm_tune_gemm: unknown code %d (20 / 21: split-K off / on)", code);
+    return DM_EINVAL;
 }
 
 extern "C" int dm_gemm(int bf16, const void* A, int64_t lda, int64_t a_batch_stride, const void* B, int64_t ldb,
@@ -1118,11 +617,8 @@ extern "C" int dm_gemm(int bf16, const void* A, int64_t lda, int64_t a_batch_str
         DM_REQUIRE(N % 64 == 0 && ldc % 8 == 0 && !ep->residual && !ep->rowvec && !ep->out_f32,
                    "GEGLU epilogue: N multiple of 64 (interleaved value/gate rows), 16-bit output of N/2 columns");
     }
-    // batched GEMMs keep per-batch tiles; only the (possibly folded) batch-1 form pairs CTAs
-    TileChoice tc = (batch == 1) ? choose_tile(M, N, K / BK, bn_hint, ep ? ep->act : 0)
-                                 : TileChoice{pick_bn((int64_t)M * batch, N, bn_hint >= 1000 ? 0 : bn_hint), false, 0};
-    const int bn = tc.bn; const bool pair = tc.pair;
-    if (ep && ep->act == 3) DM_REQUIRE(bn % 64 == 0, "GEGLU epilogue needs a tile width that is a multiple of 64");
+    TileChoice tc = choose_tile((int64_t)M * batch, N, bn_hint);
+    const int bn = tc.bn;
     CUtensorMap tmA, tmB;
     {
         uint64_t dims[3] = {(uint64_t)K, (uint64_t)M, (uint64_t)batch};
@@ -1133,7 +629,7 @@ extern "C" int dm_gemm(int bf16, const void* A, int64_t lda, int64_t a_batch_str
     {
         uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)(b_batch_stride ? batch : 1)};
         uint64_t str[2] = {(uint64_t)ldb * 2, (uint64_t)(b_batch_stride ? b_batch_stride : (int64_t)N * ldb) * 2};
-        uint32_t box[3] = {BK, (uint32_t)(pair ? bn / 2 : bn), 1}, es[3] = {1, 1, 1};
+        uint32_t box[3] = {BK, (uint32_t)bn, 1}, es[3] = {1, 1, 1};
         int rc = encode_map(&tmB, bf16, B, 3, dims, str, box, es); if (rc) return rc;
     }
     if (batch > 1 && !b_batch_stride) {
@@ -1163,34 +659,8 @@ extern "C" int dm_conv2d(int bf16, const void* x, int n_img, int H, int W, int C
     int tile_n = BM / (tile_w * tile_h);
     DM_REQUIRE(tile_w * tile_h * tile_n == BM && Wo % tile_w == 0 && Ho % tile_h == 0,
                "output extent must tile into 128-pixel boxes (power-of-two sizes)");
-    TileChoice tc = choose_tile((int64_t)n_img * Ho * Wo, Cout, ksize * ksize * Cin / BK, bn_hint, ep ? ep->act : 0);
-    if (g_gemm_halo && bn_hint == 0 && ksize == 3 && stride == 1 && pad_t == 1 && pad_l == 1 && Ho == H && Wo == W && Wo % BM == 0 &&
-        (Cout == 128 || Cout % 256 == 0) && (!ep || ep->act != 3) &&
-        dm_ceil_div((int64_t)n_img * Ho * Wo, 2 * BM) * dm_ceil_div(Cout, Cout == 128 ? 128 : 256) >= DM_NUM_SMS / 2) {
-        const int hbn = Cout == 128 ? 128 : 256;
-        CUtensorMap tmH, tmBh;
-        {
-            uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)n_img};
-            uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-            uint32_t box[4] = {BK, (uint32_t)HALO_W, 3, 1}, es[4] = {1, 1, 1, 1};
-            int rc = encode_map(&tmH, bf16, x, 4, dims, str, box, es); if (rc) return rc;
-        }
-        const int Kh = 9 * Cin;
-        {
-            uint64_t dims[3] = {(uint64_t)Kh, (uint64_t)Cout, 1};
-            uint64_t str[2] = {(uint64_t)Kh * 2, (uint64_t)Kh * Cout * 2};
-            uint32_t box[3] = {BK, (uint32_t)(hbn / 2), 1}, es[3] = {1, 1, 1};
-            int rc = encode_map(&tmBh, bf16, w, 3, dims, str, box, es); if (rc) return rc;
-        }
-        GemmParams p; memset(&p, 0, sizeof(p));
-        p.M = n_img * Ho * Wo; p.N = Cout; p.K = Kh; p.batch = 1; p.is_conv = 1; p.Cin = Cin; p.taps = 9; p.kw_n = 3;
-        p.Ho = Ho; p.Wo = Wo; p.tile_w = BM; p.tile_h = 1; p.tile_n = 1; p.stride = 1; p.pad_t = 1; p.pad_l = 1;
-        p.out = y; p.ldc = (int)ldc; p.out_batch_stride = 0;
-        fill_epilogue(p, ep, Cout);
-        return hbn == 128 ? dispatch_halo<128>(tmH, tmBh, p, bf16, (cudaStream_t)stream)
-                          : dispatch_halo<256>(tmH, tmBh, p, bf16, (cudaStream_t)stream);
-    }
-    const int bn = tc.bn; const bool pair = tc.pair;
+    TileChoice tc = choose_tile((int64_t)n_img * Ho * Wo, Cout, bn_hint);
+    const int bn = tc.bn;
     CUtensorMap tmA, tmB;
     {
         uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)n_img};
@@ -1203,7 +673,7 @@ extern "C" int dm_conv2d(int bf16, const void* x, int n_img, int H, int W, int C
     {
         uint64_t dims[3] = {(uint64_t)K, (uint64_t)Cout, 1};
         uint64_t str[2] = {(uint64_t)K * 2, (uint64_t)K * Cout * 2};
-        uint32_t box[3] = {BK, (uint32_t)(pair ? bn / 2 : bn), 1}, es[3] = {1, 1, 1};
+        uint32_t box[3] = {BK, (uint32_t)bn, 1}, es[3] = {1, 1, 1};
         int rc = encode_map(&tmB, bf16, w, 3, dims, str, box, es); if (rc) return rc;
     }
     GemmParams p; memset(&p, 0, sizeof(p));
@@ -1251,16 +721,7 @@ extern "C" int dm_conv2d_csd(int bf16, const void* x, int B, int H, int W, int C
     p.csd = 1; p.csd_B = B; p.csd_hw = hw; p.csd_groups = (int)(((int64_t)B * hw) / BM);
     p.csd_noise = c->noise; p.csd_w = c->w; p.csd_coef = c->coef;
     p.csd_grad = c->grad; p.csd_dlat = c->dlatents; p.csd_norms = c->norms; p.csd_eps = c->eps_out;
+    // persistent 64-wide kernel, one CTA per tile GROUP (three row tiles)
     cudaStream_t st = (cudaStream_t)stream;
-    // persistent single-CTA kernel, 64-wide tile, one CTA per tile GROUP (three row tiles)
-    auto launch_csd = [&](auto kern) -> int {
-        // (idempotent; the plain conv path sets the same attribute on the same instantiation)
-        DM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64, 2>::SMEM));
-        const int64_t slots = (int64_t)DM_NUM_SMS * 2;
-        const unsigned grid = (unsigned)(p.csd_groups < slots ? p.csd_groups : slots);
-        DM_CHECK_CUDA(dm_launch(kern, dim3(grid), dim3(NTHREADS), (size_t)Cfg<64, 2>::SMEM, st, tmA, tmB, p));
-        DM_CHECK_LAUNCH();
-        return DM_OK;
-    };
-    return bf16 ? launch_csd(tc_gemm_kernel<64, __nv_bfloat16, 2>) : launch_csd(tc_gemm_kernel<64, __half, 2>);
+    return bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, p, p.csd_groups, st) : launch<64, __half>(tmA, tmB, p, p.csd_groups, st);
 }

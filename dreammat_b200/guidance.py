@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's guidance plugin on top of the B200 kernels.
+"""Host-side mirror of the reference's guidance plugin on top of the H100 kernels.
 
     StableDiffusionLightGuidance  <->  threestudio `stable-diffusion-dreammat-guidance`
                                        (models/guidance/dreammat_guidance.py:44-626)

@@ -25,7 +25,7 @@ def quiesce_host_gc() -> None:
     GPU every step ends in a collective, so the step is as slow as the slowest rank's HOST, and a full generation-2 collection
     of this process takes 32-40 ms (measured) against a 25 ms 8-GPU step.  After the freeze a full collection only walks what
     was allocated since (microseconds).  Insurance, not a measured win: the 300-step A/B runs on 1 and 2 GPUs
-    (profiles/r02_exp_step_outliers.md) saw no step hit by a collection either way -- the step allocates few container objects.
+    saw no step hit by a collection either way -- the step allocates few container objects.
     No reference counterpart."""
     gc.collect()
     gc.freeze()
@@ -91,7 +91,7 @@ def warm_exchange(max_rows: int, world: int, device) -> None:
     """Run the row exchange once per message-size decade before the step loop.  NCCL sets up point-to-point channels lazily
     and uses more of them for larger messages, while the per-step counts vary with the sampled views, so a size class first
     seen inside the loop can pay a connection setup there.  A candidate for the single 350 ms step seen in one 300-step run on
-    2 GPUs (profiles/r02_exp_step_outliers.md); not separated from the allocator cause handled by
+    2 GPUs; not separated from the allocator cause handled by
     DreamMat.reserve_step_scratch()."""
     if world == 1:
         return

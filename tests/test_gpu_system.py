@@ -131,8 +131,7 @@ def test_fused_step_matches_oracle():
     assert e_rgb < 1e-3           # north_star: 1e-3 relative on rendered RGB (fp32 path)
     assert e_lr < 1e-4
     # loss_sds = 0.5 |grad|^2 / B: its relative error is at most 2x that of the SDS gradient, which in fp16 mode sits at ~1e-2
-    # (fp16 floor; the UNet is also run-to-run nondeterministic at 7e-3 through split-K / GroupNorm atomics).  Runs on the box
-    # gave 7e-4, 1.4e-3 and once more than 2e-3; the oracle's own fp16-vs-fp32 figure (floor_l) is a single noisy draw.
+    # (fp16 floor).  Measured: 7e-4, 1.4e-3 and once more than 2e-3; the oracle's own fp16-vs-fp32 figure (floor_l) is a single noisy draw.
     assert e_ls < max(4 * floor_l, 1e-2), (e_ls, floor_l)
     # fp16 mode: the parameter gradient inherits the fp16 noise of the CSD combination (the three branches nearly cancel);
     # the bound is 2x the floor the oracle itself measures between fp16 emulation and fp32.  The fp32 mode of the same

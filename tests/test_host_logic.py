@@ -128,8 +128,8 @@ def test_material_export_matches_reference_formula():
 
 
 def test_gemm_tile_plan_matches_measured_choices():
-    """dm_gemm_plan is a pure query of choose_tile(): the kernel / tile width / split-K per layer shape that the sweeps in
-    profiles/r01_tile_sweep.txt and r01_exp_splitk.txt selected (8-view batch = 24 UNet samples, one-view batch = 3)."""
+    """dm_gemm_plan is a pure query of choose_tile(): the tile width / split-K per layer shape of the H100 kernel (132 SMs;
+    8-view batch = 24 UNet samples, one-view batch = 3)."""
     import ctypes as C
     import __graft_entry__ as g
     g.build()                                   # no-op when the library is up to date
@@ -143,14 +143,14 @@ def test_gemm_tile_plan_matches_measured_choices():
 
     L.dm_gemm_set_workspace(C.c_void_p(16), L.dm_gemm_workspace_bytes())      # the query never dereferences it
     try:
-        assert plan(98304, 320, 2880) == ("pair", 160, 1)          # UNet level 0 conv, N = 320: two exact 160-wide pair tiles
-        assert plan(24576, 640, 5760) == ("pair", 256, 1)          # level 1: 256-wide pairs despite the padded third tile
-        assert plan(6144, 1280, 11520) == ("pair", 256, 1)         # level 2
-        assert plan(1536, 1280, 23040) == ("pair", 256, 2)         # 8x8 latents, 8 views: 30 pair tiles -> split-K 2
-        assert plan(192, 1280, 11520) == ("pair", 256, 14)         # 8x8 latents, one view: 5 pair tiles -> split-K 14
-        assert plan(768, 1280, 11520) == ("pair", 256, 4)          # 16x16 latents, one view
+        assert plan(98304, 320, 2880) == ("single", 128, 1)        # UNet level 0 conv, N = 320: 128-wide tiles, the third padded
+        assert plan(24576, 640, 5760) == ("single", 128, 1)        # level 1
+        assert plan(6144, 1280, 11520) == ("single", 128, 1)       # level 2: 480 tiles
+        assert plan(1536, 1280, 23040) == ("single", 64, 1)        # 8x8 latents, 8 views: 120 128-wide tiles < 132 SMs -> 64 wide
+        assert plan(192, 1280, 11520) == ("single", 64, 3)         # 8x8 latents, one view: 40 tiles -> split-K 3
+        assert plan(768, 1280, 11520) == ("single", 64, 1)         # 16x16 latents, one view: 120 tiles, nearly one per SM
         assert plan(2097152, 128, 1152) == ("single", 128, 1)      # VAE 512^2 level, N = 128
-        assert plan(98304, 2560, 320, act=3) == ("pair", 256, 1)   # FF projection with the fused GEGLU epilogue
+        assert plan(98304, 2560, 320, act=3) == ("single", 128, 1)  # FF projection with the fused GEGLU epilogue
         assert plan(192, 1280, 1280) == ("single", 64, 1)          # short K: the workspace pass would cost more than it saves
         assert plan(12288, 320, 2880) == ("single", 128, 1)        # level 0 at one view: too few tiles for 160-wide pairs
     finally:
