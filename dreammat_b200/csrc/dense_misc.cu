@@ -74,21 +74,24 @@ __device__ __forceinline__ GnIdx gn_index(int HW, int vslab, int chunks) {
     return m;
 }
 
-// Deterministic statistics: every block reduces its threads' (a, b) pairs per group in a fixed order (no shared- or
+// Deterministic statistics: every block reduces its threads' NV per-group sums in a fixed order (no shared- or
 // global-memory float atomics) and stores them in its own row of the partials (library scratch):
-// partial[((img*slabs + slab)*chunks + chunk)*2G + 2g + {0,1}].  gn_finish_kernel then adds the rows of each group in
-// (slab, chunk) order into the caller's stats[n_img*G*2], so the statistics are bit-identical from run to run.
-__device__ __forceinline__ void gn_block_partials(const float (&a)[4], const float (&b)[4], bool active, int vslab, int cpg, int G,
-                                                  int chunks, float* __restrict__ part) {
-    __shared__ float red[256][8];
+// partial[((img*slabs + slab)*chunks + chunk)*NV*G + NV*g + which].  gn_moments_kernel (forward, NV = 4) / gn_finish_kernel
+// (backward, NV = 2) then add the rows of each group in (slab, chunk) order, so the statistics are bit-identical from run to run.
+template <int NV>
+__device__ __forceinline__ void gn_block_partials(const float (&a)[NV][4], bool active, int vslab, int cpg, int G, int chunks,
+                                                  float* __restrict__ part) {
+    __shared__ float red[256][4 * NV];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) { red[threadIdx.x][2 * j] = active ? a[j] : 0.f; red[threadIdx.x][2 * j + 1] = active ? b[j] : 0.f; }
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int w = 0; w < NV; ++w) red[threadIdx.x][NV * j + w] = active ? a[w][j] : 0.f;
     __syncthreads();
     const int img = blockIdx.y, slabs = gridDim.z;
     const int g0 = (8 * (int)blockIdx.z * vslab) / cpg, g1 = (8 * ((int)blockIdx.z + 1) * vslab - 1) / cpg;
-    float* row = part + (((int64_t)img * slabs + blockIdx.z) * chunks + blockIdx.x) * 2 * G;
-    for (int i = threadIdx.x; i < 2 * (g1 - g0 + 1); i += blockDim.x) {
-        const int g = g0 + (i >> 1), which = i & 1;
+    float* row = part + (((int64_t)img * slabs + blockIdx.z) * chunks + blockIdx.x) * NV * G;
+    for (int i = threadIdx.x; i < NV * (g1 - g0 + 1); i += blockDim.x) {
+        const int g = g0 + i / NV, which = i % NV;
         // threads t = q * vslab + (v - slab start) hold channel vector v; the group's vectors are [vlo, vhi] within this slab
         const int zb = (int)blockIdx.z * vslab;
         const int vlo = max((g * cpg) / 8, zb), vhi = min(((g + 1) * cpg - 1) / 8, zb + vslab - 1);
@@ -99,11 +102,23 @@ __device__ __forceinline__ void gn_block_partials(const float (&a)[4], const flo
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const int c = 8 * v + 2 * j;         // channel pair c, c + 1 (pairs never straddle a group)
-                    if (c >= g * cpg && c < (g + 1) * cpg) acc += red[t][2 * j + which];
+                    if (c >= g * cpg && c < (g + 1) * cpg) acc += red[t][NV * j + which];
                 }
             }
-        row[2 * g + which] = acc;
+        row[NV * g + which] = acc;
     }
+}
+
+// entry i = (img*G + g)*NV + which of the per-group sums: the partial rows of group g added in (slab, chunk) order
+template <int NV>
+__device__ __forceinline__ float gn_partial_sum(const float* __restrict__ part, int i, int C, int G, int vslab, int slabs,
+                                                int chunks) {
+    const int img = i / (NV * G), r = i - img * NV * G, g = r / NV, cpg = C / G;
+    const int z0 = ((g * cpg) / 8) / vslab, z1 = (((g + 1) * cpg - 1) / 8) / vslab;
+    float acc = 0.f;
+    for (int z = z0; z <= z1; ++z)
+        for (int c = 0; c < chunks; ++c) acc += part[(((int64_t)img * slabs + z) * chunks + c) * NV * G + r];
+    return acc;
 }
 
 __global__ void __launch_bounds__(256) gn_finish_kernel(int n_img, int C, int G, int vslab, int slabs, int chunks,
@@ -112,16 +127,53 @@ __global__ void __launch_bounds__(256) gn_finish_kernel(int n_img, int C, int G,
     griddep_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_img * G * 2) return;
-    const int img = i / (2 * G), r = i - img * 2 * G, g = r >> 1, cpg = C / G;
-    const int z0 = ((g * cpg) / 8) / vslab, z1 = (((g + 1) * cpg - 1) / 8) / vslab;
-    float acc = 0.f;
-    for (int z = z0; z <= z1; ++z)
-        for (int c = 0; c < chunks; ++c) acc += part[(((int64_t)img * slabs + z) * chunks + c) * 2 * G + r];
-    stats[i] = acc;
+    stats[i] = gn_partial_sum<2>(part, i, C, G, vslab, slabs, chunks);
 }
 
-// stats[(img*G + g)*2 + {0,1}] = (sum, sumsq) over the group's channels: this kernel writes the chunk's partial row.  Channel
-// PAIRS never straddle a group (cpg is even for every SD layer), so each thread keeps 4 (sum, sumsq) pairs.
+// The one-pass variance E[x^2] - mean^2 from fp32 (sum, sumsq) loses precision as (mean / std)^2: measured on a 512x512x4
+// group, the fp16 output error is 1.04x the rounding floor at |mean| = 10 std and 26x at 100 std.  So the forward also sums
+// x - K about a pivot K per (image, group), the group's element at pixel 0, channel g*cpg; about a value drawn from the group
+// itself the cancellation is only that of (mean - K) / std.
+template <typename T>
+__device__ __forceinline__ float gn_pivot(const T* __restrict__ x, int img, int HW, int ld, int g, int cpg) {
+    return H<T>::f(x[(int64_t)img * HW * ld + g * cpg]);
+}
+
+// stats[(img*G + g)*2 + {0,1}] = (mean, rstd), the same meaning as in the fp32 mode (hp_groupnorm).  Where |mean| <= 8 std
+// (fp16 output error within ~1.02x the rounding floor) they come from the plain (sum, sumsq) by the one-pass formula
+// mean = S/cnt, var = fma(SS, 1/cnt, -mean^2), written with explicit roundings so the result does not depend on how the
+// compiler contracts it; beyond that from the pivoted sums.  The partial rows are [sum, sumsq, sum about K, sumsq about K].
+template <typename T>
+__global__ void __launch_bounds__(256) gn_moments_kernel(int n_img, int HW, int C, int ld, int G, int vslab, int slabs,
+                                                         int chunks, const float* __restrict__ part, const T* __restrict__ x,
+                                                         float eps, float* __restrict__ stats) {
+    griddep_launch_dependents();
+    griddep_wait();
+    // one thread per sum, as in gn_finish_kernel (the row loop is latency-bound: one serial chain per thread); the first lane
+    // of each group of four takes the other three sums by shuffle.  Every lane of a warp reaches the shuffles.
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool valid = i < n_img * G * 4;
+    const float s = valid ? gn_partial_sum<4>(part, i, C, G, vslab, slabs, chunks) : 0.f;
+    const float ss = __shfl_down_sync(0xffffffffu, s, 1);
+    const float sk = __shfl_down_sync(0xffffffffu, s, 2);
+    const float ssk = __shfl_down_sync(0xffffffffu, s, 3);
+    if (!valid || (i & 3)) return;
+    const int img = i / (4 * G), g = (i - img * 4 * G) >> 2, cpg = C / G;
+    const float inv_cnt = 1.0f / ((float)HW * (float)cpg);
+    const float d = sk * inv_cnt, var_k = fmaxf(ssk * inv_cnt - d * d, 0.f), mean_k = gn_pivot(x, img, HW, ld, g, cpg) + d;
+    float* o = stats + ((int64_t)img * G + g) * 2;
+    if (mean_k * mean_k > 64.f * var_k) {
+        o[0] = mean_k;
+        o[1] = rsqrtf(var_k + eps);
+    } else {
+        const float mean = __fmul_rn(s, inv_cnt);
+        o[0] = mean;
+        o[1] = rsqrtf(fmaxf(__fmaf_rn(ss, inv_cnt, -__fmul_rn(mean, mean)), 0.f) + eps);
+    }
+}
+
+// Per-thread (sum, sumsq) and (sum, sumsq) about the pivot over the group's channels: this kernel writes the chunk's partial
+// row.  Channel PAIRS never straddle a group (cpg is even for every SD layer), so each thread keeps 4 of each.
 template <typename T>
 __global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, int HW, int C, int ld, int G,
                                                        int chunks, int vslab, float* __restrict__ part) {
@@ -129,16 +181,21 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, 
     griddep_launch_dependents();
     griddep_wait();
     const GnIdx m = gn_index(HW, vslab, chunks);
-    float s[4] = {0, 0, 0, 0}, ss[4] = {0, 0, 0, 0};
+    float acc4[4][4] = {};    // [sum, sumsq, sum about K, sumsq about K][channel pair]
     if (m.active) {
         const T* base = x + ((int64_t)img * HW) * ld + 8 * m.v;
         const int lanes = m.lanes;
+        float K[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) K[j] = gn_pivot(x, img, HW, ld, (8 * m.v + 2 * j) / cpg, cpg);
         auto acc = [&](const uint4& u) {
             const T* h = reinterpret_cast<const T*>(&u);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 float a = H<T>::f(h[2 * j]), b = H<T>::f(h[2 * j + 1]);
-                s[j] += a + b; ss[j] += a * a + b * b;
+                acc4[0][j] += a + b; acc4[1][j] += a * a + b * b;
+                float ak = a - K[j], bk = b - K[j];
+                acc4[2][j] += ak + bk; acc4[3][j] += ak * ak + bk * bk;
             }
         };
         int p = m.p0 + m.q;
@@ -151,7 +208,7 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, 
         }
         for (; p < m.p1; p += lanes) acc(*reinterpret_cast<const uint4*>(base + (int64_t)p * ld));
     }
-    gn_block_partials(s, ss, m.active, vslab, cpg, G, chunks, part);
+    gn_block_partials<4>(acc4, m.active, vslab, cpg, G, chunks, part);
 }
 
 // y = act(x * A[c] + B[c]) with A = rstd*gamma, B = beta - mean*rstd*gamma (16 registers per thread).
@@ -159,11 +216,10 @@ template <typename T>
 __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, int HW, int C, int ld, int ldy, int G,
                                                        int chunks, int vslab, const float* __restrict__ stats,
                                                        const T* __restrict__ gamma, const T* __restrict__ beta,
-                                                       float eps, int silu, T* __restrict__ y) {
+                                                       int silu, T* __restrict__ y) {
     griddep_launch_dependents();
     griddep_wait();
     const int img = blockIdx.y, cpg = C / G;
-    const float inv_cnt = 1.0f / ((float)HW * (float)cpg);
     const GnIdx m = gn_index(HW, vslab, chunks);
     if (!m.active) return;
     const int v = m.v, lanes = m.lanes;
@@ -171,8 +227,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         int g = (8 * v + 2 * j) / cpg;
-        float s = stats[((int64_t)img * G + g) * 2], ss = stats[((int64_t)img * G + g) * 2 + 1];
-        float mean = s * inv_cnt, rstd = rsqrtf(fmaxf(ss * inv_cnt - mean * mean, 0.f) + eps);
+        float mean = stats[((int64_t)img * G + g) * 2], rstd = stats[((int64_t)img * G + g) * 2 + 1];
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
             float gm = H<T>::f(gamma[8 * v + 2 * j + k]);
@@ -209,14 +264,13 @@ template <typename T>
 __global__ void __launch_bounds__(256) gn_bwd_stats_kernel(const T* __restrict__ x, const T* __restrict__ dz, int HW,
                                                            int C, int G, int chunks, int vslab,
                                                            const float* __restrict__ stats, const T* __restrict__ gamma,
-                                                           const T* __restrict__ beta, float eps, int silu,
+                                                           const T* __restrict__ beta, int silu,
                                                            float* __restrict__ part) {
     griddep_launch_dependents();
     const int img = blockIdx.y, cpg = C / G;
     griddep_wait();
-    const float inv_cnt = 1.0f / ((float)HW * (float)cpg);
     const GnIdx m = gn_index(HW, vslab, chunks);
-    float a1[4] = {0, 0, 0, 0}, a2[4] = {0, 0, 0, 0};
+    float a12[2][4] = {};   // [sum(gamma*dy'), sum(gamma*dy'*xhat)][channel pair]
     if (m.active) {
         const int v = m.v, lanes = m.lanes;
         // xhat*gamma + beta = x*A + Bc;  xhat = x*rs + ms
@@ -224,9 +278,8 @@ __global__ void __launch_bounds__(256) gn_bwd_stats_kernel(const T* __restrict__
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             int g = (8 * v + 2 * j) / cpg;
-            float s = stats[((int64_t)img * G + g) * 2], ss = stats[((int64_t)img * G + g) * 2 + 1];
-            float mean = s * inv_cnt;
-            rs[j] = rsqrtf(fmaxf(ss * inv_cnt - mean * mean, 0.f) + eps);
+            float mean = stats[((int64_t)img * G + g) * 2];
+            rs[j] = stats[((int64_t)img * G + g) * 2 + 1];
             ms[j] = -mean * rs[j];
         }
 #pragma unroll
@@ -243,8 +296,8 @@ __global__ void __launch_bounds__(256) gn_bwd_stats_kernel(const T* __restrict__
                 float xv = H<T>::f(hx[k]);
                 float d = H<T>::f(hd[k]) * gm[k];
                 if (silu) d *= silu_grad(fmaf(xv, A[k], Bc[k]));
-                a1[k >> 1] += d;
-                a2[k >> 1] = fmaf(d, fmaf(xv, rs[k >> 1], ms[k >> 1]), a2[k >> 1]);
+                a12[0][k >> 1] += d;
+                a12[1][k >> 1] = fmaf(d, fmaf(xv, rs[k >> 1], ms[k >> 1]), a12[1][k >> 1]);
             }
         };
         int p = m.p0 + m.q;
@@ -258,7 +311,7 @@ __global__ void __launch_bounds__(256) gn_bwd_stats_kernel(const T* __restrict__
         for (; p < m.p1; p += lanes)
             acc(*reinterpret_cast<const uint4*>(x + base + (int64_t)p * C), *reinterpret_cast<const uint4*>(dz + base + (int64_t)p * C));
     }
-    gn_block_partials(a1, a2, m.active, vslab, cpg, G, chunks, part);
+    gn_block_partials<2>(a12, m.active, vslab, cpg, G, chunks, part);
 }
 
 // backward pass 2: dx = rstd * (gamma*dy' - (S1 + xhat*S2)/cnt)  (+ dx_add if given); same mapping as gn_apply
@@ -267,7 +320,7 @@ __global__ void __launch_bounds__(256) gn_bwd_apply_kernel(const T* __restrict__
                                                            int C, int G, int chunks, int vslab,
                                                            const float* __restrict__ stats, const float* __restrict__ bstats,
                                                            const T* __restrict__ gamma, const T* __restrict__ beta,
-                                                           float eps, int silu, const T* __restrict__ dx_add,
+                                                           int silu, const T* __restrict__ dx_add,
                                                            T* __restrict__ dx) {
     griddep_launch_dependents();
     griddep_wait();
@@ -283,9 +336,8 @@ __global__ void __launch_bounds__(256) gn_bwd_apply_kernel(const T* __restrict__
     for (int j = 0; j < 4; ++j) {
         int g = (8 * v + 2 * j) / cpg;
         int64_t si = ((int64_t)img * G + g) * 2;
-        float s = stats[si], ss = stats[si + 1];
-        float mean = s * inv_cnt;
-        rs[j] = rsqrtf(fmaxf(ss * inv_cnt - mean * mean, 0.f) + eps);
+        float mean = stats[si];
+        rs[j] = stats[si + 1];
         ms[j] = -mean * rs[j];
         float S1 = bstats[si] * inv_cnt, S2 = bstats[si + 1] * inv_cnt;
         Pq[j] = rs[j] * rs[j] * S2;
@@ -675,8 +727,8 @@ inline int gn_chunks(int n_img, int HW, int slabs, int lanes) {
 }  // namespace
 
 // partial rows of one GroupNorm call in the library scratch (at least 1 MB, so one allocation serves every layer of a model)
-static float* gn_partials(int n_img, int G, int slabs, int chunks, cudaStream_t st) {
-    size_t bytes = (size_t)2 * n_img * G * slabs * chunks * sizeof(float);
+static float* gn_partials(int nv, int n_img, int G, int slabs, int chunks, cudaStream_t st) {
+    size_t bytes = (size_t)nv * n_img * G * slabs * chunks * sizeof(float);
     if (bytes < ((size_t)1 << 20)) bytes = (size_t)1 << 20;
     return (float*)dm_scratch(DM_SCRATCH_GN, bytes, st);
 }
@@ -691,15 +743,15 @@ extern "C" int dm_groupnorm(int bf16, const void* x, int n_img, int HW, int C, i
     const int vslab = gn_vslab(C / 8), slabs = (C / 8) / vslab;
     const int chunks = gn_chunks(n_img, HW, slabs, 256 / vslab);
     const dim3 grid(chunks, n_img, slabs);
-    float* part = gn_partials(n_img, G, slabs, chunks, st);
+    float* part = gn_partials(4, n_img, G, slabs, chunks, st);
     if (!part) return DM_EDRIVER;
     DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_stats_kernel<T>, grid, dim3(256), 0, st, (const T*)x, HW, C, ld, G, chunks, vslab, part)));
     DM_CHECK_LAUNCH();
-    DM_CHECK_CUDA(dm_launch(gn_finish_kernel, dim3((unsigned)dm_ceil_div(2 * n_img * G, 256)), dim3(256), 0, st, n_img, C, G, vslab, slabs, chunks,
-                            (const float*)part, stats));
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_moments_kernel<T>, dim3((unsigned)dm_ceil_div(4 * n_img * G, 256)), dim3(256), 0, st, n_img, HW, C, ld,
+                                                G, vslab, slabs, chunks, (const float*)part, (const T*)x, eps, stats)));
     DM_CHECK_LAUNCH();
     DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_apply_kernel<T>, grid, dim3(256), 0, st, (const T*)x, HW, C, ld, ldy, G, chunks, vslab, (const float*)stats,
-                                                (const T*)gamma, (const T*)beta, eps, silu, (T*)y)));
+                                                (const T*)gamma, (const T*)beta, silu, (T*)y)));
     DM_CHECK_LAUNCH();
     return DM_OK;
 }
@@ -711,20 +763,21 @@ extern "C" int dm_groupnorm_bwd(int bf16, const void* x, const void* dz, int n_i
     if (bf16 == 2) return hp_groupnorm_bwd((const float*)x, (const float*)dz, n_img, HW, C, G, (const float*)gamma, (const float*)beta, eps, silu, stats, (const float*)dx_add, (float*)dx, stream);
     DM_REQUIRE(x && dz && gamma && beta && stats && bstats && dx, "null pointer");
     DM_REQUIRE(C % 8 == 0 && C % G == 0 && (C / G) % 2 == 0, "channel layout");
+    (void)eps;   // stats already hold (mean, rstd), as in the fp32 mode
     cudaStream_t st = (cudaStream_t)stream;
     const int vslab = gn_vslab(C / 8), slabs = (C / 8) / vslab;
     const int chunks = gn_chunks(n_img, HW, slabs, 256 / vslab);
     const dim3 grid(chunks, n_img, slabs);
-    float* part = gn_partials(n_img, G, slabs, chunks, st);
+    float* part = gn_partials(2, n_img, G, slabs, chunks, st);
     if (!part) return DM_EDRIVER;
     DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_bwd_stats_kernel<T>, grid, dim3(256), 0, st,
-                            (const T*)x, (const T*)dz, HW, C, G, chunks, vslab, stats, (const T*)gamma, (const T*)beta, eps, silu, part)));
+                            (const T*)x, (const T*)dz, HW, C, G, chunks, vslab, stats, (const T*)gamma, (const T*)beta, silu, part)));
     DM_CHECK_LAUNCH();
     DM_CHECK_CUDA(dm_launch(gn_finish_kernel, dim3((unsigned)dm_ceil_div(2 * n_img * G, 256)), dim3(256), 0, st, n_img, C, G, vslab, slabs, chunks,
                             (const float*)part, bstats));
     DM_CHECK_LAUNCH();
     DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(gn_bwd_apply_kernel<T>, grid, dim3(256), 0, st, (const T*)x, (const T*)dz, HW, C, G, chunks, vslab, stats,
-                                                (const float*)bstats, (const T*)gamma, (const T*)beta, eps, silu, (const T*)dx_add, (T*)dx)));
+                                                (const float*)bstats, (const T*)gamma, (const T*)beta, silu, (const T*)dx_add, (T*)dx)));
     DM_CHECK_LAUNCH();
     return DM_OK;
 }

@@ -270,9 +270,12 @@ int dm_hp_epilogue(const float* raw, int64_t rows, int N, int64_t rows_per_batch
 
 /* ---- streaming kernels of the dense path (NHWC; storage selected by `bf16`: 0 fp16, 1 bf16, 2 fp32; fp32 math) ---- */
 /* torch.nn.GroupNorm (+ optional SiLU) as used by diffusers ResnetBlock2D / Transformer2DModel.norm.
- * x [n_img, HW, ld] (first C channels), y [n_img, HW, ldy]; stats [n_img*G*2] receives (sum, sumsq)
- * per group and is what dm_groupnorm_bwd needs.  The statistics are bit-identical from run to run: per-block partial sums
- * (in a library-owned scratch, see DETERMINISM at the top) are added in a fixed order. */
+ * x [n_img, HW, ld] (first C channels), y [n_img, HW, ldy]; stats [n_img*G*2] receives (mean, rstd)
+ * per group in every storage mode and is what dm_groupnorm_bwd needs (whose eps is therefore unused).  In 16-bit storage
+ * a group whose |mean| exceeds 8 std takes its statistics from sums of x minus a per-group pivot taken from x, so the
+ * variance stays exact when |mean| >> std; every other group from the plain (sum, sumsq).  The
+ * statistics are bit-identical from run to run: per-block partial sums (in a library-owned scratch, see DETERMINISM at
+ * the top) are added in a fixed order. */
 int dm_groupnorm(int bf16, const void* x, int n_img, int HW, int C, int ld, int G, const void* gamma,
                  const void* beta, float eps, int silu, void* y, int ldy, float* stats, void* stream);
 /* dx = d/dx [ act(GN(x)) ] . dz (+ dx_add); x, dz, dx dense [n_img, HW, C]; bstats scratch [n_img*G*2] */
