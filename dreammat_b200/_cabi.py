@@ -60,7 +60,7 @@ SIGNATURES = {
     "dm_compact_mask": (C.c_int, [P, I64, P, P, P]),
     "dm_gather_rows": (C.c_int, [P, P, I64, C.c_int, P, P]),
     "dm_depth_normalize": (C.c_int, [P, P, I64, P, P, P]),
-    "dm_shade_mc_fwd": (C.c_int, [P, P, P, C.c_int, C.c_int] + [P] * 9 + [I64] + [P] * 13),
+    "dm_shade_mc_fwd": (C.c_int, [P, P, P, C.c_int, C.c_int] + [P] * 9 + [I64] + [P] * 12),
     "dm_shade_splitsum_fwd": (C.c_int, [P, P, C.c_int, P, C.c_int, P, C.c_int, C.c_int] + [P] * 4 + [I64] + [P] * 11),
     "dm_shade_bwd": (C.c_int, [P, P, P, P, P, F, F, I64, P, P, P]),
     "dm_envmap_pack": (C.c_int, [P, I64, P, P]),

@@ -5,9 +5,9 @@
 #include <cmath>
 #include "bvh.cuh"
 
-int g_bvh_leaf_max = 4;   // triangles per leaf (dm_tune "bvh_leaf"), 1..4
-
 namespace {
+
+constexpr int BVH_LEAF_MAX = 4;   // triangles per leaf: the leaf code stores cnt - 1 in 2 bits
 
 struct Box {
     float lo[3], hi[3];
@@ -32,7 +32,7 @@ struct Builder {
         box.init();
         Box cb; cb.init();
         for (int32_t i = first; i < first + count; ++i) { box.grow(tb[perm[i]]); cb.grow(&cent[3 * (size_t)perm[i]]); }
-        if (count <= g_bvh_leaf_max) {
+        if (count <= BVH_LEAF_MAX) {
             int32_t lf = (int32_t)leaf_order.size();
             for (int32_t i = first; i < first + count; ++i) leaf_order.push_back(perm[i]);
             return ~((lf << 2) | (count - 1));

@@ -73,7 +73,7 @@ __device__ __forceinline__ bool bvh_trace(const BvhView& bv, f3 o, f3 d, float& 
     bool alive = true;
     // "while-while" traversal: every lane first descends through internal nodes until it holds a leaf (or has
     // nothing left); the warp reconverges there, so the expensive triangle tests run with all leaf-holding lanes
-    // active instead of the ~7/32 an interleaved node/leaf loop gives (profiles/r01_launches_summary.md).
+    // active instead of the few an interleaved node/leaf loop leaves.
     while (alive) {
         while (alive && cur >= 0) {
             const float4* n = bv.nodes + (int64_t)cur * 4;

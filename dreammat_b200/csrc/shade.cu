@@ -95,7 +95,7 @@ struct PixelIn {
     float m[5], mj[5];
 };
 
-constexpr int MC_WARPS_MAX = 8;   // warps (= pixels in flight) per CTA: template parameter of shade_mc_kernel, dm_tune "mc_warps"
+constexpr int MC_WARPS = 8;   // warps (= pixels) per CTA of shade_mc_kernel
 
 struct McParams {
     dm_material_cfg cfg;
@@ -107,12 +107,7 @@ struct McParams {
     float *color, *jac, *reg_sums;
     float *albedo, *roughness, *metalness, *spec_light, *diff_light, *spec_color, *diff_color;
     uint32_t* hit_bits;
-    int skip_horizon;   // dm_tune knob
-    int frontier;       // dm_tune "mc_frontier": shared-origin traversal (see origin_frontier below)
-    int refill;         // dm_tune "mc_refill": N > 0 = batched-refill traversal, idle lanes refill when fewer than N are busy
-    int defer;          // dm_tune "mc_defer": 0 off | 1 every ray that needs a descent is compacted first (phase B of the sample loop)
-                        // | N > 1 rays whose descent exceeds N node steps are re-queued and finished together in phase B
-    const int32_t* perm;   // optional coherent visiting order of the samples ([nd] diffuse ids, then [ns] specular ids)
+    int frontier;       // dm_tune "mc_frontier": 1 shared-origin traversal (see origin_frontier below) | 0 root traversal
 };
 
 // Per-pixel quantities are warp-uniform; they live in shared memory (one record per warp) instead of being
@@ -149,7 +144,7 @@ __device__ __forceinline__ D3 spec_direction(const PixState& px, float phi0, flo
 // Each ray then runs two warp-uniform loops (local triangles, frontier boxes: broadcast loads, all lanes busy, no stack)
 // and only descends, divergently, into the frontier subtrees its own slab test hit.  The set of boxes / triangles a ray
 // can reach is exactly that of a root traversal (a box containing the origin always passes slab2), so the any-hit result
-// is bit-identical; measured effect in profiles/r02_shade_frontier.md.
+// is bit-identical.
 constexpr int FR_MAX = 64;        // frontier entries per pixel = bits of the per-ray hit mask (overflow -> plain root traversal)
 constexpr int FR_LEAF_MAX = 12;   // leaves of T_p
 constexpr float FR_INSIDE = 3e-5f;  // p must sit this far inside a box to count as contained (ray origins are p + 1e-5 d, |d| = 1)
@@ -191,57 +186,15 @@ __device__ __forceinline__ void origin_frontier(const BvhView& bv, f3 p, Frontie
     F.nl = nl;
 }
 
-// Frontier refinement (whole warp).  The warp-uniform slab loop over the frontier is ~20 instructions per box with all
-// lanes busy; a divergent node visit costs ~60 at a third of the lanes.  So the frontier is grown towards FR_MAX entries by
-// repeatedly replacing the internal node that subtends the largest solid angle from p (surface area / squared distance: the
-// box most rays hit, i.e. the one whose false positives cost most) by its two children.  Purely a re-arrangement of which
-// box tests run coherently: the reachable set of triangles is unchanged.
-__device__ __forceinline__ void refine_frontier(const BvhView& bv, f3 p, FrontierList& F, int lane, int target) {
-    int nf = F.nf;
-    if (nf < 0) return;
-    while (nf < target) {
-        float best = -1.0f; int best_i = -1;
-        for (int i = lane; i < nf; i += 32) {
-            if (F.code[i] < 0) continue;                       // leaves cannot be opened
-            const float* b = F.box[i];
-            const float ex = b[3] - b[0], ey = b[4] - b[1], ez = b[5] - b[2];
-            const float dx = fmaxf(fmaxf(b[0] - p.x, p.x - b[3]), 0.f), dy = fmaxf(fmaxf(b[1] - p.y, p.y - b[4]), 0.f),
-                        dz = fmaxf(fmaxf(b[2] - p.z, p.z - b[5]), 0.f);
-            const float m = (ex * ey + ey * ez + ez * ex) / (dx * dx + dy * dy + dz * dz + 1e-6f);
-            if (m > best) { best = m; best_i = i; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
-            if (ob > best || (ob == best && oi >= 0 && (best_i < 0 || oi < best_i))) { best = ob; best_i = oi; }
-        }
-        if (best_i < 0) break;                                 // only leaves left
-        if (lane == 0) {
-            const float4* n = bv.nodes + (int64_t)F.code[best_i] * 4;
-            const float4 n0 = __ldg(n), n1 = __ldg(n + 1), n2 = __ldg(n + 2), n3 = __ldg(n + 3);
-            float* a = F.box[best_i]; float* c = F.box[nf];
-            a[0] = n0.x; a[1] = n0.y; a[2] = n0.z; a[3] = n0.w; a[4] = n1.x; a[5] = n1.y; F.code[best_i] = __float_as_int(n3.x);
-            c[0] = n1.z; c[1] = n1.w; c[2] = n2.x; c[3] = n2.y; c[4] = n2.z; c[5] = n2.w; F.code[nf] = __float_as_int(n3.y);
-        }
-        ++nf;
-        __syncwarp();
-    }
-    if (lane == 0) F.nf = nf;
-    __syncwarp();
-}
-
-// any-hit over the frontier subtrees selected by `mask` (bit i = F.code[i]); same node / leaf steps as bvh_trace<true>.
-// Returns 0 = no hit, 1 = hit, 2 = `budget` node / leaf steps used up without a verdict (the caller re-queues the ray).
-__device__ __forceinline__ int anyhit_subtrees(const BvhView& bv, const FrontierList& F, unsigned long long mask, f3 o, f3 d,
-                                               f3 inv, f3 oi, int budget) {
+// any-hit over the frontier subtrees selected by `mask` (bit i = F.code[i]); same node / leaf steps as bvh_trace<true>
+__device__ __forceinline__ bool anyhit_subtrees(const BvhView& bv, const FrontierList& F, unsigned long long mask, f3 o, f3 d,
+                                                f3 inv, f3 oi) {
     int stack[DM_BVH_STACK];
     int sp = 0, cur = 0;
     bool alive = mask != 0ull;
     if (alive) { const int i = __ffsll((long long)mask) - 1; mask &= mask - 1ull; cur = F.code[i]; }
     while (alive) {
         while (alive && cur >= 0) {
-            if (--budget < 0) return 2;
             const float4* n = bv.nodes + (int64_t)cur * 4;
             float4 n0 = __ldg(n), n1 = __ldg(n + 1), n2 = __ldg(n + 2), n3 = __ldg(n + 3);
             float tl, tr;
@@ -266,20 +219,19 @@ __device__ __forceinline__ int anyhit_subtrees(const BvhView& bv, const Frontier
                 const float4* tp = bv.tris + (int64_t)(first + k) * 3;
                 float4 A = __ldg(tp), B = __ldg(tp + 1), C = __ldg(tp + 2);
                 float u, v;
-                if (tri_hit_pre(o, d, A, B, C, u, v) < DM_RT_MAX_DIST) return 1;
+                if (tri_hit_pre(o, d, A, B, C, u, v) < DM_RT_MAX_DIST) return true;
             }
         }
         if (sp > 0) cur = stack[--sp];
         else if (mask) { const int i = __ffsll((long long)mask) - 1; mask &= mask - 1ull; cur = F.code[i]; }
         else break;
     }
-    return 0;
+    return false;
 }
 
-// WPS = resident warps per SM the register allocation is held to: 24 (<= 85 registers, no spills) or 32 (<= 64 registers,
-// ~120 B of spills per thread; the traversal is latency-bound, so a third more warps can pay for them: dm_tune "mc_occupancy")
-template <int MC_WARPS, int WPS, bool REFILL>
-__global__ void __launch_bounds__(MC_WARPS * 32, WPS / MC_WARPS) shade_mc_kernel(McParams P) {
+// One warp per pixel.  4 CTAs (32 warps) resident per SM hold the allocation to 64 registers at the price of some spills;
+// the traversal is latency-bound and gains more from the extra warps than it loses to the spills.
+__global__ void __launch_bounds__(MC_WARPS * 32, 4) shade_mc_kernel(McParams P) {
     extern __shared__ float s_tab[];  // [nd*3 | ns*2]: (az0, sqrt(ue+1e-7), sqrt(1-ue+1e-7)) | (phi0, ue)
     __shared__ float s_in[MC_WARPS][20];
     __shared__ PixState s_px[MC_WARPS];
@@ -288,10 +240,6 @@ __global__ void __launch_bounds__(MC_WARPS * 32, WPS / MC_WARPS) shade_mc_kernel
     float* s_td = s_tab;
     float* s_ts = s_tab + 3 * nd;
     uint16_t* s_list = reinterpret_cast<uint16_t*>(s_tab + 3 * nd + 2 * ns);   // [MC_WARPS][S] compacted sample ids
-    // deferred-ray work list: [MC_WARPS][S] box masks (8-byte aligned) then [MC_WARPS][S] sample ids
-    unsigned long long* s_wl_mask = reinterpret_cast<unsigned long long*>(
-        (reinterpret_cast<uintptr_t>(s_list + MC_WARPS * S) + 7u) & ~static_cast<uintptr_t>(7));
-    unsigned short* s_wl_id = reinterpret_cast<unsigned short*>(s_wl_mask + (size_t)MC_WARPS * S);
     for (int i = threadIdx.x; i < nd; i += blockDim.x) {
         float ua = P.tab_d[2 * i], ue = P.tab_d[2 * i + 1];
         s_td[3 * i] = ua * PI_F * 2.0f;            // az = az * pi * 2 (:563)
@@ -304,379 +252,212 @@ __global__ void __launch_bounds__(MC_WARPS * 32, WPS / MC_WARPS) shade_mc_kernel
     }
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    float reg_kd_acc = 0.f, reg_ks_acc = 0.f;     // lane 0: this warp's share of the smoothness regulariser
-    // Persistent warps: warp w of the grid shades pixels w, w + W, w + 2W, ... (W = warps in the grid) with no block-level
-    // synchronisation after the table load, so a slow pixel delays only its own warp, not the seven others of its CTA
-    // (9 % of the stall samples of the one-CTA-per-8-pixels version sat in its final barrier: profiles/r02_shade_frontier.md).
-    for (int64_t pix = (int64_t)blockIdx.x * MC_WARPS + warp; pix < P.n; pix += (int64_t)gridDim.x * MC_WARPS) {
-        __syncwarp();
-        // coalesced staging of the 19 per-pixel input floats through shared memory
-        if (lane < 3) s_in[warp][lane] = P.pts[3 * pix + lane];
-        else if (lane < 6) s_in[warp][lane] = P.normals[3 * pix + lane - 3];
-        else if (lane < 9) s_in[warp][lane] = P.viewdirs[3 * pix + lane - 6];
-        else if (lane < 14) s_in[warp][lane] = P.features[5 * pix + lane - 9];
-        else if (lane < 19) s_in[warp][lane] = P.features_jitter[5 * pix + lane - 14];
-        __syncwarp();
-        const float* si = s_in[warp];
-        PixState& px = s_px[warp];
-        if (lane == 0) {
-            const f3 p = mk3(si[0], si[1], si[2]), n = mk3(si[3], si[4], si[5]), v = mk3(si[6], si[7], si[8]);
-            const float a = sigmoidf_(si[13]) * (P.cfg.max_roughness - P.cfg.min_roughness) + P.cfg.min_roughness;
-            const float ndv = dot3(v, n);
-            const f3 r = (ndv * n) * 2.0f - v;  // reflections (:620)
-            const f3 xd = ortho_dir(n), yd = cross3(n, xd), xs = ortho_dir(r), ys = cross3(r, xs);
-            const float NoV = fminf(fmaxf(ndv, 0.f), 1.f);
-            const Dual g1 = ggx_G1(mkd(NoV), mkd(a, 1.0f));
-            px.p[0] = p.x; px.p[1] = p.y; px.p[2] = p.z; px.n[0] = n.x; px.n[1] = n.y; px.n[2] = n.z;
-            px.v[0] = v.x; px.v[1] = v.y; px.v[2] = v.z; px.r[0] = r.x; px.r[1] = r.y; px.r[2] = r.z;
-            px.xd[0] = xd.x; px.xd[1] = xd.y; px.xd[2] = xd.z; px.yd[0] = yd.x; px.yd[1] = yd.y; px.yd[2] = yd.z;
-            px.xs[0] = xs.x; px.xs[1] = xs.y; px.xs[2] = xs.z; px.ys[0] = ys.x; px.ys[1] = ys.y; px.ys[2] = ys.z;
-            px.a = a; px.NoV = NoV; px.g1v = g1.v; px.g1d = g1.d;
-            px.rd = P.rand_d[pix] * PI_F * 2.0f; px.rs = P.rand_s[pix] * PI_F * 2.0f;
-            if (P.frontier) origin_frontier(P.bvh, p, s_fr[warp]);
-        }
-        __syncwarp();
-        if (P.frontier > 1) refine_frontier(P.bvh, mk3(px.p[0], px.p[1], px.p[2]), s_fr[warp], lane, P.frontier < FR_MAX ? P.frontier : FR_MAX);
-        const FrontierList& FR = s_fr[warp];
-        const bool use_frontier = P.frontier && FR.nf >= 0;
-        const float kd_pdf = (float)nd / (float)(ns + nd), ks_pdf = (float)ns / (float)(ns + nd);
+    const int64_t pix = (int64_t)blockIdx.x * MC_WARPS + warp;
+    if (pix >= P.n) return;
+    // coalesced staging of the 19 per-pixel input floats through shared memory
+    if (lane < 3) s_in[warp][lane] = P.pts[3 * pix + lane];
+    else if (lane < 6) s_in[warp][lane] = P.normals[3 * pix + lane - 3];
+    else if (lane < 9) s_in[warp][lane] = P.viewdirs[3 * pix + lane - 6];
+    else if (lane < 14) s_in[warp][lane] = P.features[5 * pix + lane - 9];
+    else if (lane < 19) s_in[warp][lane] = P.features_jitter[5 * pix + lane - 14];
+    __syncwarp();
+    const float* si = s_in[warp];
+    PixState& px = s_px[warp];
+    if (lane == 0) {
+        const f3 p = mk3(si[0], si[1], si[2]), n = mk3(si[3], si[4], si[5]), v = mk3(si[6], si[7], si[8]);
+        const float a = sigmoidf_(si[13]) * (P.cfg.max_roughness - P.cfg.min_roughness) + P.cfg.min_roughness;
+        const float ndv = dot3(v, n);
+        const f3 r = (ndv * n) * 2.0f - v;  // reflections (:620)
+        const f3 xd = ortho_dir(n), yd = cross3(n, xd), xs = ortho_dir(r), ys = cross3(r, xs);
+        const float NoV = fminf(fmaxf(ndv, 0.f), 1.f);
+        const Dual g1 = ggx_G1(mkd(NoV), mkd(a, 1.0f));
+        px.p[0] = p.x; px.p[1] = p.y; px.p[2] = p.z; px.n[0] = n.x; px.n[1] = n.y; px.n[2] = n.z;
+        px.v[0] = v.x; px.v[1] = v.y; px.v[2] = v.z; px.r[0] = r.x; px.r[1] = r.y; px.r[2] = r.z;
+        px.xd[0] = xd.x; px.xd[1] = xd.y; px.xd[2] = xd.z; px.yd[0] = yd.x; px.yd[1] = yd.y; px.yd[2] = yd.z;
+        px.xs[0] = xs.x; px.xs[1] = xs.y; px.xs[2] = xs.z; px.ys[0] = ys.x; px.ys[1] = ys.y; px.ys[2] = ys.z;
+        px.a = a; px.NoV = NoV; px.g1v = g1.v; px.g1d = g1.d;
+        px.rd = P.rand_d[pix] * PI_F * 2.0f; px.rs = P.rand_s[pix] * PI_F * 2.0f;
+        if (P.frontier) origin_frontier(P.bvh, p, s_fr[warp]);
+    }
+    __syncwarp();
+    const FrontierList& FR = s_fr[warp];
+    const bool use_frontier = P.frontier && FR.nf >= 0;
+    const float kd_pdf = (float)nd / (float)(ns + nd), ks_pdf = (float)ns / (float)(ns + nd);
 
-        float Ld[3] = {0, 0, 0}, Ls[3] = {0, 0, 0};
-        float U[3] = {0, 0, 0}, V[3] = {0, 0, 0};      // sum L*w, sum L*w*fh
-        float Ud[3] = {0, 0, 0}, Vd[3] = {0, 0, 0};    // d/da of the above with fh held fixed
-        float Wd[3] = {0, 0, 0};                       // sum L*w*dfh/da
+    float Ld[3] = {0, 0, 0}, Ls[3] = {0, 0, 0};
+    float U[3] = {0, 0, 0}, V[3] = {0, 0, 0};      // sum L*w, sum L*w*fh
+    float Ud[3] = {0, 0, 0}, Vd[3] = {0, 0, 0};    // d/da of the above with fh held fixed
+    float Wd[3] = {0, 0, 0};                       // sum L*w*dfh/da
 
-        // ---- work list.  Specular samples whose direction falls below the horizon have NoL = 0 -> G = 0 -> weight and
-        // d(weight)/da exactly 0; unless the aux light maps are requested their radiance is never used, so they are not
-        // traced.  Instead of idling their lanes, the surviving sample ids are compacted (ballot + prefix count) behind the
-        // diffuse ids, so every pass of the loop below runs with 32 live rays and there are fewer passes.
-        uint16_t* list = s_list + warp * S;
-        const bool compact = P.skip_horizon && !P.spec_light && !P.hit_bits;
-        int count;
-        if (compact) {
-            for (int i = lane; i < nd; i += 32) list[i] = (uint16_t)i;
-            count = nd;
-            for (int j0 = 0; j0 < ns; j0 += 32) {
-                const int j = j0 + lane;
-                bool act = false;
-                if (j < ns) {
-                    D3 d = spec_direction(px, s_ts[2 * j], s_ts[2 * j + 1]);
-                    act = (d.x.v * px.n[0] + d.y.v * px.n[1] + d.z.v * px.n[2]) > 0.0f;
-                }
-                const unsigned bal = __ballot_sync(0xffffffffu, act);
-                if (act) list[count + __popc(bal & ((1u << lane) - 1u))] = (uint16_t)(nd + j);
-                count += __popc(bal);
+    // ---- work list.  Specular samples whose direction falls below the horizon have NoL = 0 -> G = 0 -> weight and
+    // d(weight)/da exactly 0; unless the aux light maps are requested their radiance is never used, so they are not
+    // traced.  Instead of idling their lanes, the surviving sample ids are compacted (ballot + prefix count) behind the
+    // diffuse ids, so every pass of the loop below runs with 32 live rays and there are fewer passes.
+    uint16_t* list = s_list + warp * S;
+    const bool compact = !P.spec_light && !P.hit_bits;
+    int count;
+    if (compact) {
+        for (int i = lane; i < nd; i += 32) list[i] = (uint16_t)i;
+        count = nd;
+        for (int j0 = 0; j0 < ns; j0 += 32) {
+            const int j = j0 + lane;
+            bool act = false;
+            if (j < ns) {
+                D3 d = spec_direction(px, s_ts[2 * j], s_ts[2 * j + 1]);
+                act = (d.x.v * px.n[0] + d.y.v * px.n[1] + d.z.v * px.n[2]) > 0.0f;
             }
+            const unsigned bal = __ballot_sync(0xffffffffu, act);
+            if (act) list[count + __popc(bal & ((1u << lane) - 1u))] = (uint16_t)(nd + j);
+            count += __popc(bal);
+        }
+    } else {
+        for (int i = lane; i < S; i += 32) list[i] = (uint16_t)i;
+        count = S;
+    }
+    __syncwarp();
+    auto sample_dir = [&](int s) -> D3 {                       // sample direction (value and d/da), :554-596
+        D3 d;
+        if (s < nd) {
+            float az = s_td[3 * s] + px.rd;
+            az = az - floorf(az / TWO_PI_F) * TWO_PI_F;  // % (2 pi)
+            float sn, cs;
+            sincosf(az, &sn, &cs);
+            float cx = s_td[3 * s + 1] * cs, cy = s_td[3 * s + 1] * sn, cz = s_td[3 * s + 2];
+            d.x = mkd(cx * px.xd[0] + cy * px.yd[0] + cz * px.n[0]);
+            d.y = mkd(cx * px.xd[1] + cy * px.yd[1] + cz * px.n[1]);
+            d.z = mkd(cx * px.xd[2] + cy * px.yd[2] + cz * px.n[2]);
         } else {
-            for (int i = lane; i < S; i += 32) list[i] = (uint16_t)(P.perm ? P.perm[i] : i);
-            count = S;
+            const int j = s - nd;
+            d = spec_direction(px, s_ts[2 * j], s_ts[2 * j + 1]);
         }
-        __syncwarp();
-        // ---- per-sample pieces shared by the two phases below
-        auto sample_dir = [&](int s) -> D3 {                       // sample direction (value and d/da), :554-596
-            D3 d;
-            if (s < nd) {
-                float az = s_td[3 * s] + px.rd;
-                az = az - floorf(az / TWO_PI_F) * TWO_PI_F;  // % (2 pi)
-                float sn, cs;
-                sincosf(az, &sn, &cs);
-                float cx = s_td[3 * s + 1] * cs, cy = s_td[3 * s + 1] * sn, cz = s_td[3 * s + 2];
-                d.x = mkd(cx * px.xd[0] + cy * px.yd[0] + cz * px.n[0]);
-                d.y = mkd(cx * px.xd[1] + cy * px.yd[1] + cz * px.n[1]);
-                d.z = mkd(cx * px.xd[2] + cy * px.yd[2] + cz * px.n[2]);
-            } else {
-                const int j = s - nd;
-                d = spec_direction(px, s_ts[2 * j], s_ts[2 * j + 1]);
-            }
-            return d;
-        };
-        auto shade_sample = [&](int s, const D3& d) {             // unoccluded sample: BRDF terms (value and d/da) + env texel (:615-677)
-            const bool spec = s >= nd;
-            const f3 dv = mk3(d.x.v, d.y.v, d.z.v);
-            const f3 n = mk3(px.n[0], px.n[1], px.n[2]), v = mk3(px.v[0], px.v[1], px.v[2]);
-            const Dual aD = mkd(px.a, 1.0f);
-            D3 h; h.x = d.x + v.x; h.y = d.y + v.y; h.z = d.z + v.z;   // H = normalize(v + d) (:513-514)
-            Dual hl = dsqrt(ddot(h, h));
-            float hlc = fmaxf(hl.v, 1e-12f);
-            Dual hinv = mkd(1.0f / hlc, (hl.v > 1e-12f) ? (-hl.d / (hlc * hlc)) : 0.0f);
-            D3 Hh; Hh.x = h.x * hinv; Hh.y = h.y * hinv; Hh.z = h.z * hinv;
-            Dual HoV = dclamp01(ddot(Hh, v));
-            Dual fh = dpow5(dclamp01(1.0f - HoV));
-            Dual NoL = dclamp01(ddot(d, n));
-            Dual NoH = dclamp01(ddot(Hh, n));
-            Dual Dg = ggx_D(NoH, aD);
-            Dual G = mkd(px.g1v, px.g1d) * ggx_G1(NoL, aD);
-            Dual pdf;
-            if (!spec) pdf = mkd(NoL.v / PI_F * kd_pdf);
-            else pdf = Dg * NoH / (4.0f * HoV + 1e-5f) * ks_pdf;
-            Dual w = Dg * G / (4.0f * px.NoV * pdf + 1e-5f);
-            float4 L4 = env_fetch(P.env, P.envH, P.envW, dv);
-            const float L[3] = {L4.x, L4.y, L4.z};
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                if (!spec) Ld[c] += L[c]; else Ls[c] += L[c];
-                float lw = L[c] * w.v;
-                U[c] += lw; V[c] += lw * fh.v;
-                float lwd = L[c] * w.d;
-                Ud[c] += lwd; Vd[c] += lwd * fh.v;
-                Wd[c] += lw * fh.d;
-            }
-        };
-        auto mark_hit = [&](int s) {
-            if (P.hit_bits) atomicOr(P.hit_bits + pix * ((S + 31) / 32) + (s >> 5), 1u << (s & 31));
-        };
-        const bool horizon_cull = P.skip_horizon && !P.spec_light && !P.hit_bits;
-        if constexpr (REFILL) {
-          if (!use_frontier) {     // frontier overflow for this pixel (never seen on the bench meshes): plain root traversal
-            for (int base = 0; base < count; base += 32) {
-                if (base + lane >= count) continue;
-                const int s = list[base + lane];
-                const D3 d = sample_dir(s);
-                const f3 dv = mk3(d.x.v, d.y.v, d.z.v);
-                if (horizon_cull && s >= nd && (dv.x * px.n[0] + dv.y * px.n[1] + dv.z * px.n[2]) <= 0.0f) continue;
-                const f3 o = mk3(px.p[0] + dv.x * 1e-5f, px.p[1] + dv.y * 1e-5f, px.p[2] + dv.z * 1e-5f);
-                float bt, bu, bvv; int bid;
-                if (bvh_trace<true>(P.bvh, o, dv, bt, bid, bu, bvv)) mark_hit(s); else shade_sample(s, d);
-            }
-          } else {
-            // ---- batched-refill traversal.  The divergent descents are heavy-tailed (the slowest of 32 lanes takes ~6x the
-            // mean), which held the lock-step version at 5 / 32 active lanes there.  Here every lane carries its own ray
-            // (sample id, frontier mask, node stack); the warp descends leaf by leaf until fewer than `refill` lanes are still
-            // busy, then the idle lanes -- together -- shade / mark their finished rays, draw the next samples of the pixel
-            // and run the coherent tests (local triangles, frontier boxes) for them, and the descent resumes with a full warp.
-            int next = 0;                       // next unassigned slot of the sample list (warp-uniform)
-            int s_cur = 0, fin = 0;             // fin: 0 nothing pending, 1 finished unoccluded (shade it), 2 finished occluded
-            bool have = false;
-            unsigned long long rmask = 0ull;
-            int cur = 0, sp = 0;
-            int stack[DM_BVH_STACK];
-            f3 ro = mk3(0, 0, 0), rd3 = mk3(0, 0, 1), rinv = mk3(0, 0, 0), roi = mk3(0, 0, 0);
-            const unsigned lt = (1u << lane) - 1u;
-            while (true) {
-                // -- finished rays of the last descent, all idle lanes together
-                if (fin == 1) shade_sample(s_cur, sample_dir(s_cur));
-                else if (fin == 2) mark_hit(s_cur);
-                fin = 0;
-                // -- refill
-                const unsigned need = __ballot_sync(0xffffffffu, !have);
-                const int my = next + __popc(need & lt);
-                bool got = !have && my < count;
-                next += __popc(need);
-                if (__any_sync(0xffffffffu, got)) {
-                    const int s = got ? list[my] : 0;
-                    const D3 d = sample_dir(s);
-                    const f3 dv = mk3(d.x.v, d.y.v, d.z.v);
-                    if (got && horizon_cull && s >= nd && (dv.x * px.n[0] + dv.y * px.n[1] + dv.z * px.n[2]) <= 0.0f) got = false;
-                    const f3 o = mk3(px.p[0] + dv.x * 1e-5f, px.p[1] + dv.y * 1e-5f, px.p[2] + dv.z * 1e-5f);
-                    bool hit = false;
-                    for (int li = 0; li < FR.nl; ++li) {
-                        const int code = ~FR.leaf[li];
-                        const int first = code >> 2, cnt = (code & 3) + 1;
-                        for (int k = 0; k < cnt; ++k) {
-                            const float4* tp = P.bvh.tris + (int64_t)(first + k) * 3;
-                            const float4 A = __ldg(tp), B = __ldg(tp + 1), C = __ldg(tp + 2);
-                            float u, v;
-                            if (got && !hit && tri_hit_pre(o, dv, A, B, C, u, v) < DM_RT_MAX_DIST) hit = true;
-                        }
-                    }
-                    const f3 inv = mk3(1.0f / dv.x, 1.0f / dv.y, 1.0f / dv.z);
-                    const f3 oi = mk3(o.x * inv.x, o.y * inv.y, o.z * inv.z);
-                    unsigned long long mask = 0ull;
-                    if (got && !hit) {
-                        for (int i = 0; i < FR.nf; ++i) {
-                            float tn;
-                            if (slab2(FR.box[i][0], FR.box[i][1], FR.box[i][2], FR.box[i][3], FR.box[i][4], FR.box[i][5], inv, oi,
-                                      DM_RT_MAX_DIST, tn)) mask |= 1ull << i;
-                        }
-                    }
-                    if (got) {
-                        if (hit) mark_hit(s);
-                        else if (mask == 0ull) shade_sample(s, d);
-                        else {
-                            have = true; s_cur = s; ro = o; rd3 = dv; rinv = inv; roi = oi; sp = 0;
-                            const int i = __ffsll((long long)mask) - 1;
-                            cur = FR.code[i]; rmask = mask & (mask - 1ull);
-                        }
-                    }
-                }
-                const unsigned act0 = __ballot_sync(0xffffffffu, have);
-                if (act0 == 0u) { if (next >= count) break; continue; }
-                // -- descent, one leaf at a time, until too few lanes are busy (or to the end once the list is exhausted)
-                const int thresh = next >= count ? 1 : P.refill;
-                while (true) {
-                    if (have) {
-                        bool alive = true;
-                        while (alive && cur >= 0) {           // down to the next leaf (or out of work)
-                            const float4* n = P.bvh.nodes + (int64_t)cur * 4;
-                            float4 n0 = __ldg(n), n1 = __ldg(n + 1), n2 = __ldg(n + 2), n3 = __ldg(n + 3);
-                            float tl, tr;
-                            bool hl = slab2(n0.x, n0.y, n0.z, n0.w, n1.x, n1.y, rinv, roi, DM_RT_MAX_DIST, tl);
-                            bool hr = slab2(n1.z, n1.w, n2.x, n2.y, n2.z, n2.w, rinv, roi, DM_RT_MAX_DIST, tr);
-                            int cl = __float_as_int(n3.x), cr = __float_as_int(n3.y);
-                            if (hl && hr) {
-                                bool lfirst = tl <= tr;
-                                if (sp < DM_BVH_STACK) stack[sp++] = lfirst ? cr : cl;
-                                cur = lfirst ? cl : cr;
-                            } else if (hl) cur = cl;
-                            else if (hr) cur = cr;
-                            else if (sp > 0) cur = stack[--sp];
-                            else if (rmask) { const int i = __ffsll((long long)rmask) - 1; rmask &= rmask - 1ull; cur = FR.code[i]; }
-                            else alive = false;
-                        }
-                        if (!alive) { have = false; fin = 1; }
-                        else {
-                            const int code = ~cur;
-                            const int first = code >> 2, cnt = (code & 3) + 1;
-                            bool hit = false;
-                            for (int k = 0; k < cnt; ++k) {
-                                const float4* tp = P.bvh.tris + (int64_t)(first + k) * 3;
-                                float4 A = __ldg(tp), B = __ldg(tp + 1), C = __ldg(tp + 2);
-                                float u, v;
-                                if (tri_hit_pre(ro, rd3, A, B, C, u, v) < DM_RT_MAX_DIST) hit = true;
-                            }
-                            if (hit) { have = false; fin = 2; }
-                            else if (sp > 0) cur = stack[--sp];
-                            else if (rmask) { const int i = __ffsll((long long)rmask) - 1; rmask &= rmask - 1ull; cur = FR.code[i]; }
-                            else { have = false; fin = 1; }
-                        }
-                    }
-                    if (__popc(__ballot_sync(0xffffffffu, have)) < thresh) break;
-                }
-            }
-          }
-        } else {
-        // ---- phase A (lane = slot of the work list, all lanes in step).  Samples are visited in table order (Fibonacci points
-        // sorted by elevation).  With the frontier: local triangles and frontier boxes are tested here, coherently; a ray
-        // that is neither occluded by a local triangle nor clear of every frontier box is DEFERRED: (sample id, box mask)
-        // goes to a per-warp list in shared memory (ballot-compacted), so that phase B descends with every lane holding a
-        // ray that really needs the divergent traversal (the undeferred version ran that part at 5 of 32 lanes).
-        unsigned short* wl_id = s_wl_id + warp * S;
-        unsigned long long* wl_mask = s_wl_mask + (size_t)warp * S;
-        int wl_count = 0;
-        const bool defer = use_frontier && P.defer;
-        for (int base = 0; base < count; base += 32) {
-            const bool in_range = base + lane < count;
-            const int s = in_range ? list[base + lane] : 0;
-            const D3 d = sample_dir(s);
-            const f3 dv = mk3(d.x.v, d.y.v, d.z.v);
-            // a specular sample below the horizon has NoL = 0 -> G = 0 -> weight and d(weight)/da exactly 0: unless the
-            // aux light maps are requested its radiance is never used, so the ray need not be traced
-            const bool valid = in_range && !(horizon_cull && s >= nd && (dv.x * px.n[0] + dv.y * px.n[1] + dv.z * px.n[2]) <= 0.0f);
-            // ---- occlusion first (:490-507): occluded samples contribute nothing, skip their BRDF math
-            bool hit = false, need = false;
-            unsigned long long mask = 0ull;
-            const f3 o = mk3(px.p[0] + dv.x * 1e-5f, px.p[1] + dv.y * 1e-5f, px.p[2] + dv.z * 1e-5f);
-            if (use_frontier) {
-                // (1) the triangles around p: warp-uniform loop, broadcast loads
-                for (int li = 0; li < FR.nl; ++li) {
-                    const int code = ~FR.leaf[li];
-                    const int first = code >> 2, cnt = (code & 3) + 1;
-                    for (int k = 0; k < cnt; ++k) {
-                        const float4* tp = P.bvh.tris + (int64_t)(first + k) * 3;
-                        const float4 A = __ldg(tp), B = __ldg(tp + 1), C = __ldg(tp + 2);
-                        float u, v;
-                        if (valid && !hit && tri_hit_pre(o, dv, A, B, C, u, v) < DM_RT_MAX_DIST) hit = true;
-                    }
-                }
-                // (2) frontier boxes: warp-uniform loop over shared memory
-                const f3 inv = mk3(1.0f / dv.x, 1.0f / dv.y, 1.0f / dv.z);
-                const f3 oi = mk3(o.x * inv.x, o.y * inv.y, o.z * inv.z);
-                if (valid && !hit) {
-                    for (int i = 0; i < FR.nf; ++i) {
-                        float tn;
-                        if (slab2(FR.box[i][0], FR.box[i][1], FR.box[i][2], FR.box[i][3], FR.box[i][4], FR.box[i][5], inv, oi,
-                                  DM_RT_MAX_DIST, tn)) mask |= 1ull << i;
-                    }
-                    need = mask != 0ull;
-                }
-                if (need && (!defer || P.defer > 1)) {
-                    // (3) divergent descent right here -- P.defer > 1: for at most that many node steps; the few rays that
-                    // need more (the descent lengths are heavy-tailed: the slowest of 32 lanes takes ~6x the mean, which is
-                    // what held the warp at 5 / 32 lanes) are re-queued and finished together in phase B
-                    const int st_ = anyhit_subtrees(P.bvh, FR, mask, o, dv, inv, oi, (defer && P.defer > 1) ? P.defer : 0x7fffffff);
-                    hit = st_ == 1;
-                    need = st_ == 2;
-                }
-            } else if (valid) {
-                float bt, bu, bvv; int bid;
-                hit = bvh_trace<true>(P.bvh, o, dv, bt, bid, bu, bvv);
-            }
-            if (defer) {
-                const unsigned bal = __ballot_sync(0xffffffffu, need);
-                if (need) {
-                    const int pos = wl_count + __popc(bal & ((1u << lane) - 1u));
-                    wl_id[pos] = (unsigned short)s; wl_mask[pos] = mask;
-                }
-                wl_count += __popc(bal);
-            }
-            if (valid && hit) mark_hit(s);
-            if (valid && !hit && !need) shade_sample(s, d);
-        }
-        // ---- phase B: the deferred rays, 32 at a time, every lane with a live ray at entry
-        if (defer) {
-            __syncwarp();
-            for (int base = 0; base < wl_count; base += 32) {
-                if (base + lane >= wl_count) continue;
-                const int s = wl_id[base + lane];
-                const unsigned long long mask = wl_mask[base + lane];
-                const D3 d = sample_dir(s);
-                const f3 dv = mk3(d.x.v, d.y.v, d.z.v);
-                const f3 o = mk3(px.p[0] + dv.x * 1e-5f, px.p[1] + dv.y * 1e-5f, px.p[2] + dv.z * 1e-5f);
-                const f3 inv = mk3(1.0f / dv.x, 1.0f / dv.y, 1.0f / dv.z);
-                const f3 oi = mk3(o.x * inv.x, o.y * inv.y, o.z * inv.z);
-                if (anyhit_subtrees(P.bvh, FR, mask, o, dv, inv, oi, 0x7fffffff) == 1) mark_hit(s);
-                else shade_sample(s, d);
-            }
-        }
-        }
+        return d;
+    };
+    auto shade_sample = [&](int s, const D3& d) {             // unoccluded sample: BRDF terms (value and d/da) + env texel (:615-677)
+        const bool spec = s >= nd;
+        const f3 dv = mk3(d.x.v, d.y.v, d.z.v);
+        const f3 n = mk3(px.n[0], px.n[1], px.n[2]), v = mk3(px.v[0], px.v[1], px.v[2]);
+        const Dual aD = mkd(px.a, 1.0f);
+        D3 h; h.x = d.x + v.x; h.y = d.y + v.y; h.z = d.z + v.z;   // H = normalize(v + d) (:513-514)
+        Dual hl = dsqrt(ddot(h, h));
+        float hlc = fmaxf(hl.v, 1e-12f);
+        Dual hinv = mkd(1.0f / hlc, (hl.v > 1e-12f) ? (-hl.d / (hlc * hlc)) : 0.0f);
+        D3 Hh; Hh.x = h.x * hinv; Hh.y = h.y * hinv; Hh.z = h.z * hinv;
+        Dual HoV = dclamp01(ddot(Hh, v));
+        Dual fh = dpow5(dclamp01(1.0f - HoV));
+        Dual NoL = dclamp01(ddot(d, n));
+        Dual NoH = dclamp01(ddot(Hh, n));
+        Dual Dg = ggx_D(NoH, aD);
+        Dual G = mkd(px.g1v, px.g1d) * ggx_G1(NoL, aD);
+        Dual pdf;
+        if (!spec) pdf = mkd(NoL.v / PI_F * kd_pdf);
+        else pdf = Dg * NoH / (4.0f * HoV + 1e-5f) * ks_pdf;
+        Dual w = Dg * G / (4.0f * px.NoV * pdf + 1e-5f);
+        float4 L4 = env_fetch(P.env, P.envH, P.envW, dv);
+        const float L[3] = {L4.x, L4.y, L4.z};
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-            Ld[c] = warp_sum(Ld[c]); Ls[c] = warp_sum(Ls[c]);
-            U[c] = warp_sum(U[c]); V[c] = warp_sum(V[c]);
-            Ud[c] = warp_sum(Ud[c]); Vd[c] = warp_sum(Vd[c]); Wd[c] = warp_sum(Wd[c]);
+            if (!spec) Ld[c] += L[c]; else Ls[c] += L[c];
+            float lw = L[c] * w.v;
+            U[c] += lw; V[c] += lw * fh.v;
+            float lwd = L[c] * w.d;
+            Ud[c] += lwd; Vd[c] += lwd * fh.v;
+            Wd[c] += lw * fh.d;
         }
-        if (lane == 0) {
-            float m[5], mj[5];
-#pragma unroll
-            for (int k = 0; k < 5; ++k) { m[k] = sigmoidf_(si[9 + k]); mj[k] = sigmoidf_(si[14 + k]); }
-            // material_smoothness_grad (:110-123)
-            float k0 = fabsf(m[0] - mj[0]), k1 = fabsf(m[1] - mj[1]), k2 = fabsf(m[2] - mj[2]);
-            const float reg_kd = ((k0 + k1 + k2) / 3.0f) * k2;
-            const float reg_ks = fabsf(m[3] - mj[3]) * fabsf(m[4] - mj[4]);
-            const float alb[3] = {fminf(fmaxf(m[0], 0.f), 1.f), fminf(fmaxf(m[1], 0.f), 1.f), fminf(fmaxf(m[2], 0.f), 1.f)};
-            const float met = m[3] * (P.cfg.max_metallic - P.cfg.min_metallic) + P.cfg.min_metallic;
-            const float a = px.a;
-            const float invS = 1.0f / (float)S, invd = 1.0f / (float)nd, invs = 1.0f / (float)ns;
-            float colv[3], specv[3], diffv[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                float F0 = 0.04f * (1.0f - met) + met * alb[c];
-                float spec = (F0 * (U[c] - V[c]) + V[c]) * invS;
-                float diff = alb[c] * (Ld[c] * invd);
-                float lin = diff + spec;
-                float g = lin2srgb_grad(lin);
-                float dS_dF0 = (U[c] - V[c]) * invS;
-                float dS_da = (F0 * (Ud[c] - Vd[c]) + Vd[c] + (1.0f - F0) * Wd[c]) * invS;
-                colv[c] = lin2srgb_f(lin); specv[c] = spec; diffv[c] = diff;
-                P.jac[9 * pix + 3 * c + 0] = g * (Ld[c] * invd + dS_dF0 * met);          // d/d albedo_c
-                P.jac[9 * pix + 3 * c + 1] = g * (dS_dF0 * (alb[c] - 0.04f));            // d/d metallic
-                P.jac[9 * pix + 3 * c + 2] = g * dS_da;                                   // d/d a
+    };
+    auto mark_hit = [&](int s) {
+        if (P.hit_bits) atomicOr(P.hit_bits + pix * ((S + 31) / 32) + (s >> 5), 1u << (s & 31));
+    };
+    // ---- lane = slot of the work list, all lanes in step.  Samples are visited in table order (Fibonacci points sorted
+    // by elevation).  With the frontier, local triangles and frontier boxes are tested coherently and each ray descends
+    // only into the frontier subtrees its slab test hit.
+    for (int base = 0; base < count; base += 32) {
+        const bool in_range = base + lane < count;
+        const int s = in_range ? list[base + lane] : 0;
+        const D3 d = sample_dir(s);
+        const f3 dv = mk3(d.x.v, d.y.v, d.z.v);
+        // a specular sample below the horizon has NoL = 0 -> G = 0 -> weight and d(weight)/da exactly 0: unless the
+        // aux light maps are requested its radiance is never used, so the ray need not be traced
+        const bool valid = in_range && !(compact && s >= nd && (dv.x * px.n[0] + dv.y * px.n[1] + dv.z * px.n[2]) <= 0.0f);
+        // ---- occlusion first (:490-507): occluded samples contribute nothing, skip their BRDF math
+        bool hit = false;
+        const f3 o = mk3(px.p[0] + dv.x * 1e-5f, px.p[1] + dv.y * 1e-5f, px.p[2] + dv.z * 1e-5f);
+        if (use_frontier) {
+            // (1) the triangles around p: warp-uniform loop, broadcast loads
+            for (int li = 0; li < FR.nl; ++li) {
+                const int code = ~FR.leaf[li];
+                const int first = code >> 2, cnt = (code & 3) + 1;
+                for (int k = 0; k < cnt; ++k) {
+                    const float4* tp = P.bvh.tris + (int64_t)(first + k) * 3;
+                    const float4 A = __ldg(tp), B = __ldg(tp + 1), C = __ldg(tp + 2);
+                    float u, v;
+                    if (valid && !hit && tri_hit_pre(o, dv, A, B, C, u, v) < DM_RT_MAX_DIST) hit = true;
+                }
             }
-            st3(P.color, pix, mk3(colv[0], colv[1], colv[2]));
-            if (P.albedo) st3(P.albedo, pix, mk3(lin2srgb_f(alb[0]), lin2srgb_f(alb[1]), lin2srgb_f(alb[2])));
-            if (P.roughness) P.roughness[pix] = sqrtf(a + 1e-7f);
-            if (P.metalness) P.metalness[pix] = met;
-            if (P.spec_light) st3(P.spec_light, pix, mk3(lin2srgb_f(Ls[0] * invs), lin2srgb_f(Ls[1] * invs), lin2srgb_f(Ls[2] * invs)));
-            if (P.diff_light) st3(P.diff_light, pix, mk3(lin2srgb_f(Ld[0] * invd), lin2srgb_f(Ld[1] * invd), lin2srgb_f(Ld[2] * invd)));
-            if (P.spec_color) st3(P.spec_color, pix, mk3(lin2srgb_f(specv[0]), lin2srgb_f(specv[1]), lin2srgb_f(specv[2])));
-            if (P.diff_color) st3(P.diff_color, pix, mk3(lin2srgb_f(diffv[0]), lin2srgb_f(diffv[1]), lin2srgb_f(diffv[2])));
-            reg_kd_acc += reg_kd;
-            reg_ks_acc += reg_ks;
+            // (2) frontier boxes: warp-uniform loop over shared memory
+            const f3 inv = mk3(1.0f / dv.x, 1.0f / dv.y, 1.0f / dv.z);
+            const f3 oi = mk3(o.x * inv.x, o.y * inv.y, o.z * inv.z);
+            unsigned long long mask = 0ull;
+            if (valid && !hit) {
+                for (int i = 0; i < FR.nf; ++i) {
+                    float tn;
+                    if (slab2(FR.box[i][0], FR.box[i][1], FR.box[i][2], FR.box[i][3], FR.box[i][4], FR.box[i][5], inv, oi,
+                              DM_RT_MAX_DIST, tn)) mask |= 1ull << i;
+                }
+            }
+            // (3) divergent descent into the frontier subtrees this ray's slab test hit
+            if (mask) hit = anyhit_subtrees(P.bvh, FR, mask, o, dv, inv, oi);
+        } else if (valid) {
+            float bt, bu, bvv; int bid;
+            hit = bvh_trace<true>(P.bvh, o, dv, bt, bid, bu, bvv);
         }
+        if (valid && hit) mark_hit(s);
+        if (valid && !hit) shade_sample(s, d);
     }
-    if (lane == 0 && P.reg_sums && (reg_kd_acc != 0.f || reg_ks_acc != 0.f)) {
-        atomicAdd(P.reg_sums, reg_kd_acc);
-        atomicAdd(P.reg_sums + 1, reg_ks_acc);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        Ld[c] = warp_sum(Ld[c]); Ls[c] = warp_sum(Ls[c]);
+        U[c] = warp_sum(U[c]); V[c] = warp_sum(V[c]);
+        Ud[c] = warp_sum(Ud[c]); Vd[c] = warp_sum(Vd[c]); Wd[c] = warp_sum(Wd[c]);
+    }
+    if (lane == 0) {
+        float m[5], mj[5];
+#pragma unroll
+        for (int k = 0; k < 5; ++k) { m[k] = sigmoidf_(si[9 + k]); mj[k] = sigmoidf_(si[14 + k]); }
+        // material_smoothness_grad (:110-123)
+        float k0 = fabsf(m[0] - mj[0]), k1 = fabsf(m[1] - mj[1]), k2 = fabsf(m[2] - mj[2]);
+        const float reg_kd = ((k0 + k1 + k2) / 3.0f) * k2;
+        const float reg_ks = fabsf(m[3] - mj[3]) * fabsf(m[4] - mj[4]);
+        const float alb[3] = {fminf(fmaxf(m[0], 0.f), 1.f), fminf(fmaxf(m[1], 0.f), 1.f), fminf(fmaxf(m[2], 0.f), 1.f)};
+        const float met = m[3] * (P.cfg.max_metallic - P.cfg.min_metallic) + P.cfg.min_metallic;
+        const float a = px.a;
+        const float invS = 1.0f / (float)S, invd = 1.0f / (float)nd, invs = 1.0f / (float)ns;
+        float colv[3], specv[3], diffv[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            float F0 = 0.04f * (1.0f - met) + met * alb[c];
+            float spec = (F0 * (U[c] - V[c]) + V[c]) * invS;
+            float diff = alb[c] * (Ld[c] * invd);
+            float lin = diff + spec;
+            float g = lin2srgb_grad(lin);
+            float dS_dF0 = (U[c] - V[c]) * invS;
+            float dS_da = (F0 * (Ud[c] - Vd[c]) + Vd[c] + (1.0f - F0) * Wd[c]) * invS;
+            colv[c] = lin2srgb_f(lin); specv[c] = spec; diffv[c] = diff;
+            P.jac[9 * pix + 3 * c + 0] = g * (Ld[c] * invd + dS_dF0 * met);          // d/d albedo_c
+            P.jac[9 * pix + 3 * c + 1] = g * (dS_dF0 * (alb[c] - 0.04f));            // d/d metallic
+            P.jac[9 * pix + 3 * c + 2] = g * dS_da;                                   // d/d a
+        }
+        st3(P.color, pix, mk3(colv[0], colv[1], colv[2]));
+        if (P.albedo) st3(P.albedo, pix, mk3(lin2srgb_f(alb[0]), lin2srgb_f(alb[1]), lin2srgb_f(alb[2])));
+        if (P.roughness) P.roughness[pix] = sqrtf(a + 1e-7f);
+        if (P.metalness) P.metalness[pix] = met;
+        if (P.spec_light) st3(P.spec_light, pix, mk3(lin2srgb_f(Ls[0] * invs), lin2srgb_f(Ls[1] * invs), lin2srgb_f(Ls[2] * invs)));
+        if (P.diff_light) st3(P.diff_light, pix, mk3(lin2srgb_f(Ld[0] * invd), lin2srgb_f(Ld[1] * invd), lin2srgb_f(Ld[2] * invd)));
+        if (P.spec_color) st3(P.spec_color, pix, mk3(lin2srgb_f(specv[0]), lin2srgb_f(specv[1]), lin2srgb_f(specv[2])));
+        if (P.diff_color) st3(P.diff_color, pix, mk3(lin2srgb_f(diffv[0]), lin2srgb_f(diffv[1]), lin2srgb_f(diffv[2])));
+        if (P.reg_sums && (reg_kd != 0.f || reg_ks != 0.f)) {
+            atomicAdd(P.reg_sums, reg_kd);
+            atomicAdd(P.reg_sums + 1, reg_ks);
+        }
     }
 }
 
@@ -932,50 +713,26 @@ __global__ void envmap_pack_kernel(const float* __restrict__ rgb, int64_t n, flo
 
 }  // namespace
 
-static int g_mc_skip_horizon = 1;
-static int g_mc_frontier = 1;     // dm_tune "mc_frontier": 0 root traversal | 1 shared-origin frontier | N > 1 frontier refined to N boxes (<= 64)
-static int g_mc_persistent = 0;   // dm_tune "mc_persistent": 1 = persistent warps with a static pixel interleave (measured slower:
-                                  // per-pixel cost varies ~1:5, the hardware's CTA scheduler balances better), 0 = one CTA per MC_WARPS pixels
-static int g_mc_warps = 8;        // dm_tune "mc_warps": pixels (warps) per CTA, 1 | 2 | 4 | 8
-static int g_mc_occupancy = 32;   // dm_tune "mc_occupancy": 24 | 32 resident warps per SM (register budget 85 | 64 with ~120 B of spills): 32 measured 3-4 % faster
-static int g_mc_refill = 0;       // dm_tune "mc_refill": 0 lock-step passes | N in 1..32: per-lane rays, refill when fewer than N lanes descend
-static int g_mc_defer = 0;        // dm_tune "mc_defer": 1 = compact the rays that need the divergent descent before descending (measured
-                                  // SLOWER, 13.1 vs 9.2 ms: nearly every ray needs some descent, the lanes idle because descent lengths
-                                  // differ, not because few rays enter; kept as a knob, profiles/r02_shade_frontier.md)
-extern int g_bvh_leaf_max;
+static int g_mc_frontier = 1;     // dm_tune "mc_frontier": 1 shared-origin frontier traversal | 0 root traversal
 
-/* experiment knobs of the MC shader's traversal scheduling (not part of the reference surface) */
+/* run-time switches: "mc_frontier" (MC shader traversal, 0 | 1), "pdl" (programmatic dependent launch of the dense kernels) */
 extern "C" int dm_tune(const char* key, int value) {
     if (!key) return DM_EINVAL;
-    if (!strcmp(key, "mc_skip_horizon")) g_mc_skip_horizon = value;
-    else if (!strcmp(key, "mc_frontier")) g_mc_frontier = value;
-    else if (!strcmp(key, "mc_persistent")) g_mc_persistent = value;
-    else if (!strcmp(key, "mc_defer")) g_mc_defer = value;
-    else if (!strcmp(key, "mc_refill")) g_mc_refill = value < 0 ? 0 : (value > 32 ? 32 : value);
-    else if (!strcmp(key, "mc_occupancy")) {
-        if (value != 24 && value != 32) { dm_set_error("dm_tune mc_occupancy: 24 or 32"); return DM_EINVAL; }
-        g_mc_occupancy = value;
-    }
-    else if (!strcmp(key, "mc_warps")) {
-        if (value != 1 && value != 2 && value != 4 && value != 8) { dm_set_error("dm_tune mc_warps: 1, 2, 4 or 8"); return DM_EINVAL; }
-        g_mc_warps = value;
+    if (!strcmp(key, "mc_frontier")) {
+        if (value != 0 && value != 1) { dm_set_error("dm_tune mc_frontier: 0 or 1"); return DM_EINVAL; }
+        g_mc_frontier = value;
     }
     else if (!strcmp(key, "pdl")) g_dm_pdl = value ? 1 : 0;
-    else if (!strcmp(key, "bvh_leaf")) g_bvh_leaf_max = value < 1 ? 1 : (value > 4 ? 4 : value);
-    else if (!strcmp(key, "mc_refill") || !strcmp(key, "mc_leaf_batch")) { /* retired experiment knobs */ }
     else { dm_set_error("dm_tune: unknown key %s", key); return DM_EINVAL; }
     return DM_OK;
 }
-
-static int launch_mc(const McParams& P, cudaStream_t st);
 
 extern "C" int dm_shade_mc_fwd(const dm_material_cfg* cfg, const dm_bvh* bvh, const float* env_rgba, int envH, int envW,
                                const float* tab_d, const float* tab_s, const float* pts, const float* normals,
                                const float* viewdirs, const float* features, const float* features_jitter,
                                const float* rand_d, const float* rand_s, int64_t n, float* color, float* jac,
                                float* reg_sums, float* albedo, float* roughness, float* metalness, float* spec_light,
-                               float* diff_light, float* spec_color, float* diff_color, uint32_t* hit_bits,
-                               const int32_t* sample_perm, void* stream) {
+                               float* diff_light, float* spec_color, float* diff_color, uint32_t* hit_bits, void* stream) {
     if (n == 0) return DM_OK;
     DM_REQUIRE(cfg && bvh && env_rgba && tab_d && tab_s && pts && normals && viewdirs && features && features_jitter &&
                    rand_d && rand_s && color && jac, "null pointer");
@@ -986,57 +743,17 @@ extern "C" int dm_shade_mc_fwd(const dm_material_cfg* cfg, const dm_bvh* bvh, co
     P.pts = pts; P.normals = normals; P.viewdirs = viewdirs; P.features = features; P.features_jitter = features_jitter;
     P.rand_d = rand_d; P.rand_s = rand_s; P.n = n; P.color = color; P.jac = jac; P.reg_sums = reg_sums;
     P.albedo = albedo; P.roughness = roughness; P.metalness = metalness; P.spec_light = spec_light;
-    P.diff_light = diff_light; P.spec_color = spec_color; P.diff_color = diff_color; P.hit_bits = hit_bits; P.perm = sample_perm;
-    P.skip_horizon = g_mc_skip_horizon;
+    P.diff_light = diff_light; P.spec_color = spec_color; P.diff_color = diff_color; P.hit_bits = hit_bits;
     P.frontier = g_mc_frontier;
-    P.defer = g_mc_defer;
-    P.refill = g_mc_refill;
-    return launch_mc(P, (cudaStream_t)stream);
-}
-
-namespace {
-template <int W, int WPS, bool RF = false>
-int launch_mc_w(const McParams& P, cudaStream_t st) {
-    // direction tables + one compacted sample-id list per warp (+ the deferred-ray work list when that mode is on)
-    const size_t S_ = (size_t)(P.cfg.n_diffuse + P.cfg.n_specular);
-    const size_t smem = (size_t)(3 * P.cfg.n_diffuse + 2 * P.cfg.n_specular) * sizeof(float) + (size_t)W * S_ * sizeof(uint16_t) + 8 +
-                        (P.defer ? (size_t)W * S_ * (sizeof(unsigned long long) + sizeof(unsigned short)) : 0);
+    // direction tables + one compacted sample-id list per warp
+    const size_t smem = (size_t)(3 * cfg->n_diffuse + 2 * cfg->n_specular) * sizeof(float) +
+                        (size_t)MC_WARPS * (cfg->n_diffuse + cfg->n_specular) * sizeof(uint16_t);
     static size_t smem_configured = 0;
     if (smem > smem_configured) {
-        DM_CHECK_CUDA(cudaFuncSetAttribute(shade_mc_kernel<W, WPS, RF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DM_CHECK_CUDA(cudaFuncSetAttribute(shade_mc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         smem_configured = smem;
     }
-    int64_t blocks = dm_ceil_div(P.n, W);
-    if (g_mc_persistent) {
-        static int per_sm = 0;
-        if (!per_sm) {
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, shade_mc_kernel<W, WPS, RF>, W * 32, smem) != cudaSuccess || per_sm < 1) {
-                cudaGetLastError(); per_sm = 2;
-            }
-        }
-        const int64_t resident = (int64_t)DM_NUM_SMS * per_sm;
-        if (blocks > resident) blocks = resident;
-    }
-    shade_mc_kernel<W, WPS, RF><<<(unsigned)blocks, W * 32, smem, st>>>(P);
-    return DM_OK;
-}
-}  // namespace
-
-static int launch_mc(const McParams& P, cudaStream_t st) {
-    int rc;
-    if (g_mc_refill > 0 && g_mc_frontier > 0) {
-        rc = g_mc_occupancy == 32 ? launch_mc_w<8, 32, true>(P, st) : launch_mc_w<8, 24, true>(P, st);
-    } else if (g_mc_occupancy == 32) {
-        rc = g_mc_warps == 4 ? launch_mc_w<4, 32>(P, st) : launch_mc_w<8, 32>(P, st);
-    } else {
-        switch (g_mc_warps) {
-            case 1: rc = launch_mc_w<1, 24>(P, st); break;
-            case 2: rc = launch_mc_w<2, 24>(P, st); break;
-            case 4: rc = launch_mc_w<4, 24>(P, st); break;
-            default: rc = launch_mc_w<8, 24>(P, st); break;
-        }
-    }
-    if (rc) return rc;
+    shade_mc_kernel<<<(unsigned)dm_ceil_div(n, MC_WARPS), MC_WARPS * 32, smem, (cudaStream_t)stream>>>(P);
     DM_CHECK_LAUNCH();
     return DM_OK;
 }

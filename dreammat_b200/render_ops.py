@@ -178,27 +178,6 @@ def direction_tables(n: int) -> torch.Tensor:
     return torch.from_numpy(np.stack([az * 0.5 / np.pi, 1 - 2 * el / np.pi], -1).astype(np.float32))
 
 
-def sample_order(n_diffuse: int, n_specular: int) -> torch.Tensor:
-    """Direction-coherent visiting order of the light samples for dm_shade_mc_fwd's `sample_perm`.
-
-    Both sample families are Fibonacci points on a (warped) hemisphere about the local axis, rotated by ONE random
-    azimuth per pixel, so their arrangement in the local tangent frame is fixed.  Ordering them along a Morton curve
-    of the projected disk coordinates makes each warp (32 consecutive samples) trace a compact cone instead of
-    32 directions spread over the hemisphere; the sums the shader forms are order-independent."""
-    def order(tab):
-        ua, ue = tab[:, 0].double().numpy(), tab[:, 1].double().numpy()
-        r = np.sqrt(np.clip(ue, 0, 1))
-        x, y = r * np.cos(2 * np.pi * ua), r * np.sin(2 * np.pi * ua)
-        qx = np.clip(((x + 1) * 0.5 * 255).astype(np.int64), 0, 255)
-        qy = np.clip(((y + 1) * 0.5 * 255).astype(np.int64), 0, 255)
-        code = np.zeros_like(qx)
-        for b in range(8):
-            code |= ((qx >> b) & 1) << (2 * b) | ((qy >> b) & 1) << (2 * b + 1)
-        return np.argsort(code, kind="stable")
-    pd, ps = order(direction_tables(n_diffuse)), order(direction_tables(n_specular))
-    return torch.from_numpy(np.concatenate([pd, n_diffuse + ps]).astype(np.int32))
-
-
 def envmap_pack(rgb: torch.Tensor) -> torch.Tensor:
     rgb = _f32c(rgb)
     H, W, _ = rgb.shape
@@ -222,7 +201,7 @@ def _alloc_aux(n, dev, want):
 class _ShadeMC(torch.autograd.Function):
     @staticmethod
     def forward(ctx, features, features_jitter, pts, normals, viewdirs, rand_d, rand_s, state, want_aux, reg_weight_n):
-        cfg, bvh, env_rgba, tab_d, tab_s, perm = state
+        cfg, bvh, env_rgba, tab_d, tab_s = state
         n = features.shape[0]
         dev = features.device
         features, features_jitter = _f32c(features), _f32c(features_jitter)
@@ -234,7 +213,7 @@ class _ShadeMC(torch.autograd.Function):
         check(lib().dm_shade_mc_fwd(C.byref(cfg), bvh.h, ptr(env_rgba), H, W, ptr(tab_d), ptr(tab_s), ptr(_f32c(pts)),
                                     ptr(_f32c(normals)), ptr(_f32c(viewdirs)), ptr(features), ptr(features_jitter),
                                     ptr(_f32c(rand_d).view(-1)), ptr(_f32c(rand_s).view(-1)), n, ptr(color), ptr(jac),
-                                    ptr(reg), *[ptr(a) for a in aux], None, ptr(perm), stream_ptr()), "dm_shade_mc_fwd")
+                                    ptr(reg), *[ptr(a) for a in aux], None, stream_ptr()), "dm_shade_mc_fwd")
         ctx.save_for_backward(features, features_jitter, jac)
         ctx.cfg = cfg
         ctx.inv_n = 1.0 / float(reg_weight_n if reg_weight_n else max(n, 1))
@@ -257,9 +236,9 @@ class _ShadeMC(torch.autograd.Function):
 
 
 def shade_mc(features, features_jitter, pts, normals, viewdirs, rand_d, rand_s, cfg, bvh, env_rgba, tab_d, tab_s,
-             want_aux=True, reg_weight_n=None, perm=None):
+             want_aux=True, reg_weight_n=None):
     out = _ShadeMC.apply(features, features_jitter, pts, normals, viewdirs, rand_d, rand_s,
-                         (cfg, bvh, env_rgba, tab_d, tab_s, perm), want_aux, reg_weight_n)
+                         (cfg, bvh, env_rgba, tab_d, tab_s), want_aux, reg_weight_n)
     color, reg = out[0], out[1]
     aux = dict(zip(AUX_KEYS, out[2:])) if want_aux else {}
     return color, reg, aux

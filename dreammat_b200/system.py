@@ -200,10 +200,9 @@ class DreamMatMaterial:
         self.light = [R.envmap_pack(m.to(self.device)) for m in (env_maps or [])]
         self.tab_d = R.direction_tables(c.diffuse_sample_num).to(self.device)
         self.tab_s = R.direction_tables(c.specular_sample_num).to(self.device)
-        # visiting order of the samples: identity = the Fibonacci tables' own order, sorted by elevation, so the 32 rays of a
-        # lock-step pass have similar traversal lengths.  Direction-coherent orders (R.sample_order, azimuth sectors) measured
-        # ~10 % slower (scripts/exp_shade_order.py).
-        self.perm = None
+        # the shader visits the samples in the tables' own order, sorted by elevation, so the 32 rays of a lock-step pass
+        # have similar traversal lengths; direction-coherent orders (Morton, azimuth sectors) measured slower
+        # (scripts/exp_shade_order.py)
         self.mc_cfg = MaterialCfg(c.min_metallic, c.max_metallic, c.min_roughness_squre, c.max_roughness_squre,
                                   c.diffuse_sample_num, c.specular_sample_num)
         self.ss_cfg = MaterialCfg(c.min_metallic, c.max_metallic, c.min_roughness, c.max_roughness,
@@ -250,7 +249,7 @@ class DreamMatMaterial:
             if rand_s is None:
                 rand_s = torch.rand(n, device=self.device)           # appendix B #6
             color, reg, aux = R.shade_mc(features, features_jitter, pts, normals, viewdirs, rand_d, rand_s, self.mc_cfg,
-                                         self.bvh, self.light[e], self.tab_d, self.tab_s, want_aux, reg_weight_n, self.perm)
+                                         self.bvh, self.light[e], self.tab_d, self.tab_s, want_aux, reg_weight_n)
         else:
             dcube, mips = self.envlight[e]
             color, reg, aux = R.shade_splitsum(features, features_jitter, normals, viewdirs, self.ss_cfg, self.FG_LUT,
@@ -537,7 +536,7 @@ class DreamMat:
                 check(lib().dm_shade_mc_fwd(C.byref(mat.mc_cfg), ren.ray_tracer.h, ptr(env), env.shape[0], env.shape[1],
                                             ptr(mat.tab_d), ptr(mat.tab_s), ptr(pts), ptr(nrm), ptr(vd), ptr(f),
                                             ptr(fj), ptr(rd), ptr(rs), n, ptr(color), ptr(jac), ptr(reg_sums), *([None] * 7),
-                                            None, ptr(mat.perm), st), "dm_shade_mc_fwd")
+                                            None, st), "dm_shade_mc_fwd")
             else:   # use_raytracing=false: split-sum shading (dreammat_material.py:679-711), three texture lookups per pixel
                 dcube, mips = mat.envlight[env_id]
                 check(lib().dm_shade_splitsum_fwd(C.byref(mat.ss_cfg), ptr(mat.FG_LUT), mat.FG_LUT.shape[0], ptr(dcube), dcube.shape[1],

@@ -36,8 +36,9 @@ extern "C" {
 
 const char* dm_last_error(void);
 int dm_version(void);
-/* experiment knobs (no reference counterpart): "mc_skip_horizon" (0|1 skip below-horizon specular rays), "bvh_leaf" (1..4
- * triangles per BVH leaf, takes effect at the next dm_bvh_build), "pdl" (0|1 programmatic dependent launch of the dense kernels) */
+/* run-time switches (no reference counterpart): "mc_frontier" (1 shared-origin frontier traversal of the MC shader's
+ * occlusion rays | 0 plain root traversal, the reference the frontier is tested against), "pdl" (0|1 programmatic
+ * dependent launch of the dense kernels).  Any other key or value returns DM_EINVAL. */
 int dm_tune(const char* key, int value);
 int dm_tune_attention(int mode);       /* softmax variant: 0 fp32 exponentials, rescale every block (the only one) */
 /* split-K scratch: a caller-owned device buffer of fp32 partial tiles, one slice per split, added in a fixed order by the
@@ -128,16 +129,13 @@ typedef struct {
  * Outputs: color [n,3] (sRGB, differentiable), jac [n,9] = d color_c / d (albedo_c, metallic, a)
  * for c=0..2, reg_sums[2] += (sum luma*|dkd_b|, sum |dks0|*|dks1|); aux pointers may be NULL:
  * albedo[n,3] roughness[n] metalness[n] spec_light[n,3] diff_light[n,3] spec_color[n,3] diff_color[n,3].
- * hit_bits (optional, zero-initialised by the caller): [n, ceil((nd+ns)/32)] occlusion bit per sample id.
- * sample_perm (optional): visiting order of the sample ids (a permutation of 0..nd-1 followed by one of
- * nd..nd+ns-1); sums are order-independent, a direction-coherent order cuts BVH traversal divergence. */
+ * hit_bits (optional, zero-initialised by the caller): [n, ceil((nd+ns)/32)] occlusion bit per sample id. */
 int dm_shade_mc_fwd(const dm_material_cfg* cfg, const dm_bvh* bvh, const float* env_rgba, int envH, int envW,
                     const float* tab_d, const float* tab_s, const float* pts, const float* normals,
                     const float* viewdirs, const float* features, const float* features_jitter,
                     const float* rand_d, const float* rand_s, int64_t n, float* color, float* jac,
                     float* reg_sums, float* albedo, float* roughness, float* metalness, float* spec_light,
-                    float* diff_light, float* spec_color, float* diff_color, uint32_t* hit_bits,
-                    const int32_t* sample_perm, void* stream);
+                    float* diff_light, float* spec_color, float* diff_color, uint32_t* hit_bits, void* stream);
 
 /* Split-sum shading, dreammat_material.py:679-711.  fg_lut [256,256,2]; diffuse_cube [6,rd,rd,3];
  * spec_mips: n_mips device pointers (host array) to [6,r_i,r_i,3], r_i = spec_res0 >> i. */

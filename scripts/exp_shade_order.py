@@ -40,7 +40,7 @@ for vid in (3, 40):
         td = mat.tab_d[torch.from_numpy(od[name]).to(dev)].contiguous(); ts = mat.tab_s[torch.from_numpy(os_[name]).to(dev)].contiguous()
         def run():
             return R.shade_mc(f, fj, g["pts"], g["nrm"], g["vd"], rd, rs, mat.mc_cfg, ren.ray_tracer, mat.light[0], td, ts,
-                              want_aux=False, perm=None)[0]
+                              want_aux=False)[0]
         for _ in range(2): col = run()
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -39,6 +39,14 @@ def test_missing_library_fails_loudly(monkeypatch):
         _cabi.lib()
 
 
+def test_dm_tune_accepts_only_its_switches():
+    from dreammat_b200._cabi import lib
+    assert lib().dm_tune(b"mc_frontier", 2) == -1
+    for key in (b"mc_skip_horizon", b"bvh_leaf", b"no_such_key"):
+        assert lib().dm_tune(key, 1) == -1, key
+    assert lib().dm_tune(b"mc_frontier", 1) == 0 and lib().dm_tune(b"pdl", 1) == 0   # the defaults
+
+
 def test_host_side_layout_queries():
     from dreammat_b200 import render_ops as ops
     cfg = ops.default_hashgrid_cfg()
