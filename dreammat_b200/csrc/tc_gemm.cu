@@ -14,12 +14,14 @@
 //                         Stride-2 convs use the map's element strides.
 //   * B = weights [N, K] (K-major), K index = tap * Cin + c.
 //
-// tc_gemm_kernel<BN,T>: persistent, warp-specialised, one CTA per SM walking 128 x BN output tiles.  CTA = 288 threads:
-// warps 0-7 are two consumer warpgroups (rows 0-63 / 64-127 of the tile, m64nBNk16 wgmma with both operands in shared
-// memory), warp 8 is the TMA producer.  Operand tiles live in the 128-byte swizzled K-major layout shared by TMA and the
-// wgmma descriptors; a ring of mbarrier-guarded stages lets the producer run ahead across tile boundaries.  After the K
-// loop the accumulators go through a shared-memory staging tile so the epilogue (fused bias / per-image vector / residual
-// / SiLU / GELU / GEGLU / scale -> 16-byte global stores, or a split-K partial tile) reads whole output rows.
+// tc_gemm_kernel<BN,T>: persistent, warp-specialised, one CTA per SM walking 128 x BN output tiles.  CTA = 544 threads:
+// warps 0-7 are two MMA warpgroups (rows 0-63 / 64-127 of the tile, m64nBNk16 wgmma with both operands in shared
+// memory), warps 8-15 are two epilogue warpgroups (two threads per tile row), warp 16 is the TMA producer.  Operand tiles
+// live in the 128-byte swizzled K-major layout shared by TMA and the wgmma descriptors; a ring of mbarrier-guarded stages
+// lets the producer run ahead across tile boundaries.  After a tile's K loop the MMA warpgroups hand the accumulators to
+// the epilogue warpgroups through a shared-memory staging tile (mbarriers epi_full / epi_empty) and start the next tile's
+// K loop at once, so the epilogue (fused bias / per-image vector / residual / SiLU / GELU / GEGLU / scale -> 16-byte
+// global stores, or a split-K partial tile), which reads whole output rows, overlaps the next tile's loads and MMAs.
 // choose_tile() picks the tile width and split-K.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -30,8 +32,9 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int CONSUMERS = 256;                 // two warpgroups
-constexpr int NTHREADS = CONSUMERS + 32;       // + the TMA producer warp
+constexpr int MMA_THREADS = 256;                              // two MMA warpgroups
+constexpr int EPI_THREADS = 2 * BM;                           // two epilogue warpgroups: two threads per tile row
+constexpr int NTHREADS = MMA_THREADS + EPI_THREADS + 32;      // + the TMA producer warp
 
 struct GemmParams {
     int M, N, K;                  // GEMM view; conv: M = n_img*Ho*Wo, K = taps*Cin
@@ -285,9 +288,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
     const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;
     float* epi = reinterpret_cast<float*>(smem_raw + (smem_base - raw_u32) + C::STAGES * C::STAGE_BYTES);
     const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES + C::EPI_BYTES;
-    // barriers: full[STAGES] (TMA bytes landed), empty[STAGES] (both warpgroups done reading)
+    // barriers: full[STAGES] (TMA bytes landed), empty[STAGES] (both MMA warpgroups done reading), epi_full (the staging
+    // tile holds a tile's accumulators), epi_empty (the epilogue warpgroup has finished reading them)
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
+    const uint32_t epi_full = bar_base + 16u * C::STAGES, epi_empty = epi_full + 8u;
 
     griddep_launch_dependents();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -301,12 +306,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
         prefetch_tmap(&tmA);
         prefetch_tmap(&tmB);
         for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
+        mbar_init(epi_full, MMA_THREADS / 32);      // one arrival per warp (lane 0, after __syncwarp)
+        mbar_init(epi_empty, EPI_THREADS / 32);
         fence_mbar_init();
     }
     __syncthreads();
     griddep_wait();      // PDL: everything above overlapped the previous kernel's tail; its outputs are visible from here
 
-    if (warp == CONSUMERS / 32) {
+    if (warp == (MMA_THREADS + EPI_THREADS) / 32) {
         if (lane == 0) {
             // ------------------------------------------------ TMA producer
             const int slabs = p.is_conv ? (p.Cin / BK) : nk;
@@ -343,18 +350,38 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
         }
         return;
     }
-    // -------------------------------------------------------- consumer warpgroups 0 / 1: MMA, then the epilogue
+    uint32_t epi_phase = 0;
+    if (threadIdx.x >= MMA_THREADS) {
+        // ---------------------------------------------------- epilogue warpgroups: threads row and row + 128 share a tile row
+        const int row = threadIdx.x & (BM - 1), half = (threadIdx.x - MMA_THREADS) >> 7;
+        const float* er = epi + row * C::EPI_LD;
+        const int step = p.act == 3 ? 64 : 32;
+        float csd_e[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+        for (int i = 0, t; (t = tile_at(p, i, blockIdx.x, gridDim.x, total_tiles)) >= 0; ++i) {
+            const int sp = t % S, tt = t / S;
+            const int z = tt / tiles_per_z, r_ = tt - z * tiles_per_z;
+            const int m_tile = r_ / n_tiles, n_tile = r_ - m_tile * n_tiles;
+            const int64_t m = (int64_t)m_tile * BM + row;
+            mbar_wait(epi_full, epi_phase);
+            if (BN == 64 && p.csd) {
+                if (half == 0) epilogue_csd<T>(p, er, m, lane, csd_e);     // csd_e carries a pixel's branches
+            } else {
+                epilogue_row<BN, T>(p, er, m, z, sp, n_tile, half * step, 2 * step);   // GEGLU chunks are 64 wide
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(epi_empty);
+            epi_phase ^= 1u;
+        }
+        return;
+    }
+    // -------------------------------------------------------- MMA warpgroups 0 / 1
     const int wg = warp >> 2;
     const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // accumulator fragment rows frag_row, frag_row + 8
     const int frag_col = 2 * (lane & 3);
-    const int ep_row = threadIdx.x & (BM - 1), ep_half = threadIdx.x >> 7;
     int stage = 0; uint32_t phase = 0;
-    float csd_e[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
     float acc[BN / 2];
     for (int i = 0, t; (t = tile_at(p, i, blockIdx.x, gridDim.x, total_tiles)) >= 0; ++i) {
-        const int sp = t % S, tt = t / S;
-        const int z = tt / tiles_per_z, r_ = tt - z * tiles_per_z;
-        const int m_tile = r_ / n_tiles, n_tile = r_ - m_tile * n_tiles;
+        const int sp = t % S;
         const int kb0 = (int)((int64_t)sp * nk / S), kb1 = (int)((int64_t)(sp + 1) * nk / S);
 #pragma unroll
         for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
@@ -377,24 +404,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
         wgmma_wait<0>();
         wgmma_fence_operands(acc);
         if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev));
-        named_bar_sync(1, CONSUMERS);              // the previous tile's epilogue has finished reading the staging tile
+        mbar_wait(epi_empty, epi_phase ^ 1u);      // the epilogue warpgroups have finished reading the previous tile
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
             *reinterpret_cast<float2*>(epi + frag_row * C::EPI_LD + 8 * j + frag_col) = make_float2(acc[4 * j], acc[4 * j + 1]);
             *reinterpret_cast<float2*>(epi + (frag_row + 8) * C::EPI_LD + 8 * j + frag_col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
-        named_bar_sync(1, CONSUMERS);
-        const int64_t m = (int64_t)m_tile * BM + ep_row;
-        const float* er = epi + ep_row * C::EPI_LD;
-        if constexpr (BN == 64) {
-            if (p.csd) {
-                if (ep_half == 0) epilogue_csd<T>(p, er, m, lane, csd_e);
-                continue;
-            }
-        }
-        // the two threads of a row split its column chunks (GEGLU chunks are 64 wide)
-        const int step = p.act == 3 ? 64 : 32;
-        epilogue_row<BN, T>(p, er, m, z, sp, n_tile, ep_half * step, 2 * step);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(epi_full);
+        epi_phase ^= 1u;
     }
 }
 
