@@ -20,8 +20,9 @@
 // live in the 128-byte swizzled K-major layout shared by TMA and the wgmma descriptors; a ring of mbarrier-guarded stages
 // lets the producer run ahead across tile boundaries.  After a tile's K loop the MMA warpgroups hand the accumulators to
 // the epilogue warpgroups through a shared-memory staging tile (mbarriers epi_full / epi_empty) and start the next tile's
-// K loop at once, so the epilogue (fused bias / per-image vector / residual / SiLU / GELU / GEGLU / scale -> 16-byte
-// global stores, or a split-K partial tile), which reads whole output rows, overlaps the next tile's loads and MMAs.
+// K loop at once, so the epilogue (fused bias / per-image vector / residual / SiLU / GELU / GEGLU / scale, or a split-K
+// partial tile), which reads whole output rows, overlaps the next tile's loads and MMAs.  A 16-bit output moves by TMA:
+// residual boxes are loaded into a shared output tile, combined in place and stored as boxes (see the epilogue role).
 // choose_tile() picks the tile width and split-K.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -45,6 +46,7 @@ struct GemmParams {
     int stride, pad_t, pad_l;
     // epilogue
     void* out; int ldc; int64_t out_batch_stride; int out_f32;
+    int tma_out;                  // 16-bit output (and residual) tiles move by TMA through shared memory (see dispatch)
     const void* bias;                       // [N]
     const void* rowvec; int rows_per_vec; int ld_rowvec;   // [M / rows_per_vec, N]
     const void* residual; int ld_res; int64_t res_batch_stride;
@@ -77,20 +79,50 @@ template <> struct Cvt<__nv_bfloat16> {
     static __device__ __forceinline__ __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
 };
 
-__device__ __forceinline__ void ld_row32(const float* er, int c0, float (&f)[32]) {
+// The fp32 staging tile has BN floats per row, without padding.  Its 16-byte chunks are XOR-swizzled by the row
+// (chunk ^ epi_swz(row)), so that both the MMA warps' fragment stores (rows r..r+3 x 8 columns per half-warp) and the
+// epilogue's row reads (8 consecutive rows per quarter-warp) touch 32 distinct banks.
+__device__ __forceinline__ int epi_swz(int row) { const int k = row & 7; return ((k & 3) << 1) | (k >> 2); }
+__device__ __forceinline__ int epi_idx(int row, int col) { return ((((col >> 2) ^ epi_swz(row))) << 2) + (col & 3); }
+
+// R staging columns c0 .. c0 + R - 1 of the row starting at `er`, whose swizzle is sw
+template <int R>
+__device__ __forceinline__ void ld_row(const float* er, int sw, int c0, float (&f)[R]) {
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        const float4 t = reinterpret_cast<const float4*>(er + c0)[q];
+    for (int q = 0; q < R / 4; ++q) {
+        const float4 t = reinterpret_cast<const float4*>(er)[((c0 >> 2) + q) ^ sw];
         f[4 * q] = t.x; f[4 * q + 1] = t.y; f[4 * q + 2] = t.z; f[4 * q + 3] = t.w;
     }
 }
 
-// Epilogue of one output row of a 128 x BN tile: `er` is the row's fp32 accumulator in the staging tile; this thread
-// handles the column chunks c0 = c_first, c_first + c_step, ... (32 wide, 64 for GEGLU):
-// acc*alpha + bias + rowvec -> act -> + residual -> * out_scale -> 16-byte stores.
+// The 16-bit output tile in shared memory (TMA path): BN / 32 boxes of 128 rows x 32 columns (8 KB each, 64 bytes per
+// row) in the TMA map's 64-byte swizzle.  Byte offset of 16-byte chunk q (columns 8q .. 8q + 7) of `row` in a box; the
+// 8 rows of a quarter-warp hit 8 distinct bank groups.
+constexpr int OBOX_BYTES = BM * 64;
+__device__ __forceinline__ int obox_off(int row, int q) { return row * 64 + ((q ^ ((row >> 1) & 3)) << 4); }
+
+// f[j] += vec[n0 + j] for the 8 columns n0 .. n0 + 7; columns >= N are skipped
+template <typename T>
+__device__ __forceinline__ void add8(float* f, const T* vec, int n0, int N) {
+    if (n0 + 8 <= N && ((uintptr_t)(vec + n0) & 15) == 0) {
+        const uint4 u = __ldg(reinterpret_cast<const uint4*>(vec + n0));
+        const T* h = reinterpret_cast<const T*>(&u);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] += Cvt<T>::to_f(h[j]);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) if (n0 + j < N) f[j] += Cvt<T>::to_f(vec[n0 + j]);
+    }
+}
+
+// Epilogue of one output row of a 128 x BN tile: `er` is the row's fp32 accumulator in the staging tile (swizzle sw);
+// this thread handles the column chunks c0 = c_first, c_first + c_step, ... (32 wide, 64 for GEGLU):
+// acc*alpha + bias + rowvec -> act -> + residual -> * out_scale -> 16-bit output.  On the TMA path (p.tma_out) the
+// residual is read from, and the output written to, the shared output tile `ot` (row `row` of each 32-column box); the
+// caller stores the boxes.  Otherwise both go straight to global memory with 16-byte accesses where aligned.
 template <int BN, typename T>
-__device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* er, int64_t m, int z, int sp, int n_tile,
-                                             int c_first, int c_step) {
+__device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* er, int sw, uint8_t* ot, int row, int64_t m,
+                                             int z, int sp, int n_tile, int c_first, int c_step) {
     const bool row_ok = m < p.M;
     if (!row_ok) return;
     if (p.ws) {
@@ -103,7 +135,7 @@ __device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* e
             const int n0 = n_tile * BN + c0;
             if (n0 >= p.N) continue;
             float v[32];
-            ld_row32(er, c0, v);
+            ld_row<32>(er, sw, c0, v);
             if (n0 + 32 <= p.N && (p.N & 3) == 0) {
 #pragma unroll
                 for (int q = 0; q < 8; ++q)
@@ -127,22 +159,26 @@ __device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* e
         for (int c0 = c_first; c0 < BN; c0 += c_step) {
             const int n0 = n_tile * BN + c0;
             if (n0 >= p.N) continue;
-            float v[32], g[32];
-            ld_row32(er, c0, v);
-            ld_row32(er, c0 + 32, g);
             T* o = reinterpret_cast<T*>(outp) + (n0 >> 1);
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
+                float a[8], b[8];
+                ld_row<8>(er, sw, c0 + 8 * q, a);
+                ld_row<8>(er, sw, c0 + 32 + 8 * q, b);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) { a[j] *= p.alpha; b[j] *= p.alpha; }
+                if (bias) { add8(a, bias, n0 + q * 8, p.N); add8(b, bias, n0 + 32 + q * 8, p.N); }
                 uint4 u;
                 T* h = reinterpret_cast<T*>(&u);
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int c = q * 8 + j;
-                    float a = v[c] * p.alpha, b = g[c] * p.alpha;
-                    if (bias) { a += Cvt<T>::to_f(bias[n0 + c]); b += Cvt<T>::to_f(bias[n0 + 32 + c]); }
-                    h[j] = Cvt<T>::from_f(a * (0.5f * b * (1.0f + erff(b * 0.70710678118654752f))) * p.out_scale);
+                for (int j = 0; j < 8; ++j)
+                    h[j] = Cvt<T>::from_f(a[j] * (0.5f * b[j] * (1.0f + erff(b[j] * 0.70710678118654752f))) * p.out_scale);
+                if (p.tma_out) *reinterpret_cast<uint4*>(ot + (c0 >> 6) * OBOX_BYTES + obox_off(row, q)) = u;
+                else if ((p.ldc & 7) == 0) reinterpret_cast<uint4*>(o)[q] = u;
+                else {
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) o[8 * q + j] = h[j];
                 }
-                reinterpret_cast<uint4*>(o)[q] = u;
             }
         }
         return;
@@ -152,17 +188,17 @@ __device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* e
         const int n0 = n_tile * BN + c0;
         if (n0 >= p.N) continue;
         float f[32];
-        ld_row32(er, c0, f);
+        ld_row<32>(er, sw, c0, f);
 #pragma unroll
         for (int j = 0; j < 32; ++j) f[j] *= p.alpha;
         const bool full = (n0 + 32 <= p.N);
         if (bias) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) if (full || n0 + j < p.N) f[j] += Cvt<T>::to_f(bias[n0 + j]);
+            for (int q = 0; q < 4; ++q) add8(f + 8 * q, bias, n0 + 8 * q, p.N);
         }
         if (rowvec) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) if (full || n0 + j < p.N) f[j] += Cvt<T>::to_f(rowvec[n0 + j]);
+            for (int q = 0; q < 4; ++q) add8(f + 8 * q, rowvec, n0 + 8 * q, p.N);
         }
         if (p.act == 1) {
 #pragma unroll
@@ -170,6 +206,29 @@ __device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* e
         } else if (p.act == 2) {
 #pragma unroll
             for (int j = 0; j < 32; ++j) f[j] = 0.5f * f[j] * (1.0f + erff(f[j] * 0.70710678118654752f));
+        }
+        uint8_t* obox = ot + (c0 >> 5) * OBOX_BYTES;
+        if (p.tma_out) {
+            // residual chunks were loaded into the box by TMA (zeros past N / M); each chunk is read and then
+            // overwritten with the output by this thread, and the box store clips to [M, N]
+            if (res) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const uint4 u = *reinterpret_cast<const uint4*>(obox + obox_off(row, q));
+                    const T* h = reinterpret_cast<const T*>(&u);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) f[q * 8 + j] += Cvt<T>::to_f(h[j]);
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                uint4 u;
+                T* h = reinterpret_cast<T*>(&u);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) h[j] = Cvt<T>::from_f(f[q * 8 + j] * p.out_scale);
+                *reinterpret_cast<uint4*>(obox + obox_off(row, q)) = u;
+            }
+            continue;
         }
         if (res) {
             if (full && ((p.ld_res & 7) == 0)) {
@@ -265,15 +324,15 @@ __device__ __forceinline__ void epilogue_csd(const GemmParams& p, const float* e
     }
 }
 
-// ~128 KB operand ring + the fp32 staging tile of the epilogue (row pitch BN + 4 floats: conflict-free row reads).
+// ~128 KB operand ring + the fp32 staging tile of the epilogue (swizzled, see epi_idx) + the 16-bit output tile.
 template <int BN> struct Cfg {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int STAGES = 131072 / STAGE_BYTES;        // 4 (BN = 128) or 5 (BN = 64)
-    static constexpr int EPI_LD = BN + 4;
-    static constexpr int EPI_BYTES = BM * EPI_LD * 4;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int EPI_BYTES = BM * BN * 4;
+    static constexpr int OUT_BYTES = (BN / 32) * OBOX_BYTES;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + EPI_BYTES + OUT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
 
@@ -281,18 +340,24 @@ template <int BN> struct Cfg {
 template <int BN, typename T>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
                                                              const __grid_constant__ CUtensorMap tmB,
+                                                             const __grid_constant__ CUtensorMap tmO,
+                                                             const __grid_constant__ CUtensorMap tmR,
                                                              const GemmParams p) {
     using C = Cfg<BN>;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;
     float* epi = reinterpret_cast<float*>(smem_raw + (smem_base - raw_u32) + C::STAGES * C::STAGE_BYTES);
-    const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES + C::EPI_BYTES;
+    uint8_t* otile = reinterpret_cast<uint8_t*>(epi) + C::EPI_BYTES;
+    const uint32_t otile_u32 = smem_base + C::STAGES * C::STAGE_BYTES + C::EPI_BYTES;
+    const uint32_t bar_base = otile_u32 + C::OUT_BYTES;
     // barriers: full[STAGES] (TMA bytes landed), empty[STAGES] (both MMA warpgroups done reading), epi_full (the staging
-    // tile holds a tile's accumulators), epi_empty (the epilogue warpgroup has finished reading them)
+    // tile holds a tile's accumulators), epi_empty (the epilogue warpgroups have finished reading them), res_full[2]
+    // (TMA path: epilogue warpgroup h's boxes of the output tile are free and hold the tile's residual, if any)
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
     const uint32_t epi_full = bar_base + 16u * C::STAGES, epi_empty = epi_full + 8u;
+    auto res_full = [&](int h) { return epi_full + 16u + 8u * h; };
 
     griddep_launch_dependents();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -305,9 +370,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
     if (threadIdx.x == 0) {
         prefetch_tmap(&tmA);
         prefetch_tmap(&tmB);
+        if (p.tma_out) {
+            prefetch_tmap(&tmO);
+            if (p.residual) prefetch_tmap(&tmR);
+        }
         for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
         mbar_init(epi_full, MMA_THREADS / 32);      // one arrival per warp (lane 0, after __syncwarp)
         mbar_init(epi_empty, EPI_THREADS / 32);
+        mbar_init(res_full(0), 1);
+        mbar_init(res_full(1), 1);
         fence_mbar_init();
     }
     __syncthreads();
@@ -354,8 +425,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
     if (threadIdx.x >= MMA_THREADS) {
         // ---------------------------------------------------- epilogue warpgroups: threads row and row + 128 share a tile row
         const int row = threadIdx.x & (BM - 1), half = (threadIdx.x - MMA_THREADS) >> 7;
-        const float* er = epi + row * C::EPI_LD;
+        const int sw = epi_swz(row);
+        const float* er = epi + row * BN;
         const int step = p.act == 3 ? 64 : 32;
+        // TMA path: warpgroup `half` owns the output boxes of its chunks c0 = half * step + 2 * step * k (box c0 / step;
+        // GEGLU writes 32 outputs per 64-column chunk) and runs their round trip: its leader thread loads the residual
+        // boxes of a tile into shared memory, the warpgroup adds them in place, the leader stores the boxes and, once
+        // the store has read them, loads the next tile's residual (or just releases the boxes when there is none).
+        const bool leader = (threadIdx.x & 127) == 0;
+        const uint32_t rbar = res_full(half);
+        auto fill = [&](int t) {
+            const int z = (t / S) / tiles_per_z, r_ = (t / S) - z * tiles_per_z;
+            const int m_tile = r_ / n_tiles, n_tile = r_ - m_tile * n_tiles;
+            if (!p.residual) { mbar_arrive(rbar); return; }
+            uint32_t bytes = 0;
+            for (int c0 = half * step; c0 < BN; c0 += 2 * step) if (n_tile * BN + c0 < p.N) bytes += OBOX_BYTES;
+            mbar_expect_tx(rbar, bytes);
+            for (int c0 = half * step; c0 < BN; c0 += 2 * step)
+                if (n_tile * BN + c0 < p.N) tma_load_3d(otile_u32 + (c0 / step) * OBOX_BYTES, &tmR, rbar, n_tile * BN + c0, m_tile * BM, z);
+        };
+        uint32_t res_phase = 0;
+        if (p.tma_out && leader) {
+            const int t0 = tile_at(p, 0, blockIdx.x, gridDim.x, total_tiles);
+            if (t0 >= 0) fill(t0);
+        }
         float csd_e[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
         for (int i = 0, t; (t = tile_at(p, i, blockIdx.x, gridDim.x, total_tiles)) >= 0; ++i) {
             const int sp = t % S, tt = t / S;
@@ -363,15 +456,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
             const int m_tile = r_ / n_tiles, n_tile = r_ - m_tile * n_tiles;
             const int64_t m = (int64_t)m_tile * BM + row;
             mbar_wait(epi_full, epi_phase);
+            if (p.tma_out) mbar_wait(rbar, res_phase);
             if (BN == 64 && p.csd) {
-                if (half == 0) epilogue_csd<T>(p, er, m, lane, csd_e);     // csd_e carries a pixel's branches
+                if (half == 0) epilogue_csd<T>(p, er + (sw << 2), m, lane, csd_e);     // csd_e carries a pixel's branches
             } else {
-                epilogue_row<BN, T>(p, er, m, z, sp, n_tile, half * step, 2 * step);   // GEGLU chunks are 64 wide
+                epilogue_row<BN, T>(p, er, sw, otile, row, m, z, sp, n_tile, half * step, 2 * step);   // GEGLU chunks are 64 wide
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(epi_empty);
             epi_phase ^= 1u;
+            if (p.tma_out) {
+                fence_proxy_async_smem();
+                named_bar_sync(1 + half, 128);
+                if (leader) {
+                    const int n_out0 = p.act == 3 ? (n_tile * BN) / 2 : n_tile * BN;
+                    for (int c0 = half * step; c0 < BN; c0 += 2 * step)
+                        if (n_tile * BN + c0 < p.N) tma_store_3d(&tmO, otile_u32 + (c0 / step) * OBOX_BYTES, n_out0 + (c0 / step) * 32, m_tile * BM, z);
+                    bulk_commit();
+                    bulk_wait_read();
+                    const int tn = tile_at(p, i + 1, blockIdx.x, gridDim.x, total_tiles);
+                    if (tn >= 0) fill(tn);
+                }
+                res_phase ^= 1u;
+            }
         }
+        if (p.tma_out && leader) bulk_wait_all();     // dependent kernels (PDL) read the output
         return;
     }
     // -------------------------------------------------------- MMA warpgroups 0 / 1
@@ -407,8 +516,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
         mbar_wait(epi_empty, epi_phase ^ 1u);      // the epilogue warpgroups have finished reading the previous tile
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
-            *reinterpret_cast<float2*>(epi + frag_row * C::EPI_LD + 8 * j + frag_col) = make_float2(acc[4 * j], acc[4 * j + 1]);
-            *reinterpret_cast<float2*>(epi + (frag_row + 8) * C::EPI_LD + 8 * j + frag_col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+            *reinterpret_cast<float2*>(epi + frag_row * BN + epi_idx(frag_row, 8 * j + frag_col)) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(epi + (frag_row + 8) * BN + epi_idx(frag_row + 8, 8 * j + frag_col)) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(epi_full);
@@ -435,14 +544,14 @@ EncodeTiledFn get_encode() {
 }
 
 int encode_map(CUtensorMap* m, int bf16, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-               const uint32_t* box, const uint32_t* estr) {
+               const uint32_t* box, const uint32_t* estr, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
     EncodeTiledFn fn = get_encode();
     if (!fn) { dm_set_error("cuTensorMapEncodeTiled unavailable"); return DM_EDRIVER; }
     cuuint64_t gd[5]; cuuint64_t gs[4]; cuuint32_t bx[5]; cuuint32_t es[5];
     for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bx[i] = box[i]; es[i] = estr[i]; }
     for (int i = 0; i < rank - 1; ++i) gs[i] = strides_bytes[i];
     CUresult r = fn(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank,
-                    const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                    const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         dm_set_error("cuTensorMapEncodeTiled failed (%d) rank=%d dims=%llu,%llu,%llu,%llu box=%u,%u,%u,%u", (int)r, rank,
@@ -454,8 +563,23 @@ int encode_map(CUtensorMap* m, int bf16, const void* base, int rank, const uint6
     return DM_OK;
 }
 
+// A 16-bit [batch][M][ld] output or residual is addressable by TMA when its base and strides are multiples of 16 bytes.
+int64_t out_batch_pitch(int M, int batch, int64_t ld, int64_t batch_stride) { return batch > 1 ? batch_stride : (int64_t)M * ld; }
+bool tma_addressable(const void* base, int M, int batch, int64_t ld, int64_t batch_stride) {
+    const int64_t zs = out_batch_pitch(M, batch, ld, batch_stride);
+    return ((uintptr_t)base & 15) == 0 && (ld & 7) == 0 && (zs & 7) == 0 && zs > 0;
+}
+// its 3-D map [batch][M][n] for the TMA epilogue: 128 x 32 boxes in the 64-byte swizzle of obox_off
+int out_map(CUtensorMap* m, int bf16, const void* base, int n, int M, int batch, int64_t ld, int64_t batch_stride) {
+    uint64_t dims[3] = {(uint64_t)n, (uint64_t)M, (uint64_t)batch};
+    uint64_t str[2] = {(uint64_t)ld * 2, (uint64_t)out_batch_pitch(M, batch, ld, batch_stride) * 2};
+    uint32_t box[3] = {32, BM, 1}, es[3] = {1, 1, 1};
+    return encode_map(m, bf16, base, 3, dims, str, box, es, CU_TENSOR_MAP_SWIZZLE_64B);
+}
+
 template <int BN, typename T>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int64_t work_items, cudaStream_t st) {
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR,
+           const GemmParams& p, int64_t work_items, cudaStream_t st) {
     static bool configured = false;
     auto kern = tc_gemm_kernel<BN, T>;
     if (!configured) {
@@ -463,7 +587,7 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, 
         configured = true;
     }
     unsigned grid = (unsigned)(work_items < DM_NUM_SMS ? work_items : DM_NUM_SMS);   // persistent: one CTA per SM
-    DM_CHECK_CUDA(dm_launch(kern, dim3(grid), dim3(NTHREADS), (size_t)Cfg<BN>::SMEM, st, tmA, tmB, p));
+    DM_CHECK_CUDA(dm_launch(kern, dim3(grid), dim3(NTHREADS), (size_t)Cfg<BN>::SMEM, st, tmA, tmB, tmO, tmR, p));
     DM_CHECK_LAUNCH();
     return DM_OK;
 }
@@ -566,10 +690,24 @@ int dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p
     const int split = tc.split >= 1 ? tc.split : pick_split(tiles, p.K / BK, batch * p.M * p.N, p.N, p.act);
     p.split_k = split;
     p.ws = split > 1 ? g_ws : nullptr;
-    const int64_t work = tiles * split;
+    // The epilogue moves 16-bit output and residual tiles by TMA, except for fp32 output, split-K partial tiles and
+    // rows whose pitch TMA cannot address; those keep per-thread global loads and stores.
+    CUtensorMap tmO, tmR;
+    memset(&tmO, 0, sizeof(tmO)); memset(&tmR, 0, sizeof(tmR));
+    p.tma_out = split <= 1 && !p.out_f32 && tma_addressable(p.out, p.M, (int)batch, p.ldc, p.out_batch_stride) &&
+                (!p.residual || tma_addressable(p.residual, p.M, (int)batch, p.ld_res, p.res_batch_stride));
     int rc;
-    if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, p, work, st) : launch<64, __half>(tmA, tmB, p, work, st);
-    else rc = bf16 ? launch<128, __nv_bfloat16>(tmA, tmB, p, work, st) : launch<128, __half>(tmA, tmB, p, work, st);
+    if (p.tma_out) {
+        rc = out_map(&tmO, bf16, p.out, p.act == 3 ? p.N / 2 : p.N, p.M, (int)batch, p.ldc, p.out_batch_stride);
+        if (rc) return rc;
+        if (p.residual) {
+            rc = out_map(&tmR, bf16, p.residual, p.N, p.M, (int)batch, p.ld_res, p.res_batch_stride);
+            if (rc) return rc;
+        }
+    }
+    const int64_t work = tiles * split;
+    if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half>(tmA, tmB, tmO, tmR, p, work, st);
+    else rc = bf16 ? launch<128, __nv_bfloat16>(tmA, tmB, tmO, tmR, p, work, st) : launch<128, __half>(tmA, tmB, tmO, tmR, p, work, st);
     if (rc || split <= 1) return rc;
     const int64_t n4 = batch * p.M * (p.N >> 2);
     int64_t blocks = dm_ceil_div(n4, 256);
@@ -632,7 +770,7 @@ extern "C" int dm_gemm(int bf16, const void* A, int64_t lda, int64_t a_batch_str
     DM_REQUIRE((((uintptr_t)A | (uintptr_t)B) & 15) == 0, "16-byte aligned operands");
     if (batch < 1) batch = 1;
     if (ep && ep->act == 3) {
-        DM_REQUIRE(N % 64 == 0 && ldc % 8 == 0 && !ep->residual && !ep->rowvec && !ep->out_f32,
+        DM_REQUIRE(N % 64 == 0 && !ep->residual && !ep->rowvec && !ep->out_f32,
                    "GEGLU epilogue: N multiple of 64 (interleaved value/gate rows), 16-bit output of N/2 columns");
     }
     TileChoice tc = choose_tile((int64_t)M * batch, N, bn_hint);
@@ -741,5 +879,8 @@ extern "C" int dm_conv2d_csd(int bf16, const void* x, int B, int H, int W, int C
     p.csd_grad = c->grad; p.csd_dlat = c->dlatents; p.csd_norms = c->norms; p.csd_eps = c->eps_out;
     // persistent 64-wide kernel, one CTA per tile GROUP (three row tiles)
     cudaStream_t st = (cudaStream_t)stream;
-    return bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, p, p.csd_groups, st) : launch<64, __half>(tmA, tmB, p, p.csd_groups, st);
+    CUtensorMap none;      // the CSD epilogue writes fp32 per thread: no output / residual maps
+    memset(&none, 0, sizeof(none));
+    return bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, none, none, p, p.csd_groups, st)
+                : launch<64, __half>(tmA, tmB, none, none, p, p.csd_groups, st);
 }
