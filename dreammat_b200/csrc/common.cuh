@@ -15,11 +15,11 @@ void dm_set_error(const char* fmt, ...);
 void dm_count_launch();
 
 // Library-owned device scratch of the deterministic reductions (GroupNorm partial rows, the hash-grid backward's fixed-point
-// accumulator): one buffer per device and slot, zero-filled when allocated.  Callers of one device must not use a slot from
-// two streams at once (the same rule as the split-K workspace).  A buffer is never freed, because a captured CUDA graph may
-// hold its address; it can only grow outside stream capture (a warm-up call before capture sizes it).  Returns nullptr with
-// the error set on failure.
-enum { DM_SCRATCH_GN = 0, DM_SCRATCH_HASHGRID = 1, DM_SCRATCH_AA = 2, DM_SCRATCH_SLOTS = 3 };
+// accumulator, the bias-gradient partial rows of the weight gradients): one buffer per device and slot, zero-filled when
+// allocated.  Callers of one device must not use a slot from two streams at once (the same rule as the split-K workspace).
+// A buffer is never freed, because a captured CUDA graph may hold its address; it can only grow outside stream capture (a
+// warm-up call before capture sizes it).  Returns nullptr with the error set on failure.
+enum { DM_SCRATCH_GN = 0, DM_SCRATCH_HASHGRID = 1, DM_SCRATCH_AA = 2, DM_SCRATCH_WGRAD = 3, DM_SCRATCH_SLOTS = 4 };
 void* dm_scratch(int slot, size_t bytes, cudaStream_t st);
 
 #define DM_CHECK_CUDA(expr)                                                          \

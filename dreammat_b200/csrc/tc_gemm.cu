@@ -24,6 +24,9 @@
 // partial tile), which reads whole output rows, overlaps the next tile's loads and MMAs.  A 16-bit output moves by TMA:
 // residual boxes are loaded into a shared output tile, combined in place and stored as boxes (see the epilogue role).
 // choose_tile() picks the tile width and split-K.
+//
+// Weight gradients (dm_conv2d_wgrad / dm_gemm_wgrad) run the same kernel in its WG mode: D[Cout, taps*Cin] (fp32) reduces
+// over the pixel / token axis, with both operands MN-major boxes of the NHWC / token-major dY and x (see WG_BOX).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -336,8 +339,16 @@ template <int BN> struct Cfg {
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
 
+// Weight-gradient mode (WG): D[M' = Cout, N' = taps*Cin] = sum over K' = pixels (tokens) of dY[K', M'] . x_tap[K', N'].
+// Both operands are MN-major: a stage holds 64 pixels (one K-block) of each, as 64-channel TMA boxes of 64 rows x 128 B
+// straight from the NHWC / token-major buffers: two boxes of dY (the 128 rows of the tile, one per MMA warpgroup) and
+// BN / 64 boxes of x, each loaded at its own tap's shifted origin.  Out-of-bounds pixels (padding, the ragged end of the
+// pixel axis) are zero-filled by TMA in both operands.
+constexpr int WG_BOX = 64 * 128;                     // bytes of one 64-channel x 64-pixel box
+constexpr int WG_PIX = 64;                           // pixels per K-block
+
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...
-template <int BN, typename T>
+template <int BN, typename T, bool WG = false>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
                                                              const __grid_constant__ CUtensorMap tmB,
                                                              const __grid_constant__ CUtensorMap tmO,
@@ -385,7 +396,42 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
     griddep_wait();      // PDL: everything above overlapped the previous kernel's tail; its outputs are visible from here
 
     if (warp == (MMA_THREADS + EPI_THREADS) / 32) {
-        if (lane == 0) {
+        if (lane == 0 && WG) {
+            // ------------------------------------------------ TMA producer, weight-gradient mode
+            const int tiles_w = p.is_conv ? p.Wo / p.tile_w : 1, tiles_h = p.is_conv ? p.Ho / p.tile_h : 1;
+            int stage = 0; uint32_t phase = 0;
+            for (int i = 0, t; (t = tile_at(p, i, blockIdx.x, gridDim.x, total_tiles)) >= 0; ++i) {
+                const int sp = t % S, r = t / S;
+                const int m_tile = r / n_tiles, n_tile = r - m_tile * n_tiles;
+                const int kb0 = (int)((int64_t)sp * nk / S), kb1 = (int)((int64_t)(sp + 1) * nk / S);
+                // boxes wholly past Cout / N' are not loaded: they would only feed rows / columns the epilogue drops
+                const int a_boxes = min(2, (p.M - m_tile * BM + 63) / 64), b_boxes = min(BN / 64, (p.N - n_tile * BN + 63) / 64);
+                for (int kb = kb0; kb < kb1; ++kb) {
+                    mbar_wait(empty_bar(stage), phase ^ 1u);
+                    const uint32_t a_dst = smem_base + stage * C::STAGE_BYTES;
+                    const uint32_t b_dst = a_dst + C::A_BYTES;
+                    mbar_expect_tx(full_bar(stage), (uint32_t)(a_boxes + b_boxes) * WG_BOX);
+                    if (p.is_conv) {
+                        const int tw = kb % tiles_w, th = (kb / tiles_w) % tiles_h, tn = kb / (tiles_w * tiles_h);
+                        const int ow0 = tw * p.tile_w, oh0 = th * p.tile_h, n0 = tn * p.tile_n;
+                        for (int h = 0; h < a_boxes; ++h)
+                            tma_load_4d(a_dst + h * WG_BOX, &tmA, full_bar(stage), m_tile * BM + 64 * h, ow0, oh0, n0);
+                        for (int j = 0; j < b_boxes; ++j) {
+                            // a 128-wide tile may straddle two taps: each 64-channel box takes its own tap's shift
+                            const int col = n_tile * BN + 64 * j, tap = col / p.Cin, kh = tap / p.kw_n, kw = tap - kh * p.kw_n;
+                            tma_load_4d(b_dst + j * WG_BOX, &tmB, full_bar(stage), col - tap * p.Cin,
+                                        ow0 * p.stride - p.pad_l + kw, oh0 * p.stride - p.pad_t + kh, n0);
+                        }
+                    } else {
+                        for (int h = 0; h < a_boxes; ++h)
+                            tma_load_3d(a_dst + h * WG_BOX, &tmA, full_bar(stage), m_tile * BM + 64 * h, kb * WG_PIX, 0);
+                        for (int j = 0; j < b_boxes; ++j)
+                            tma_load_3d(b_dst + j * WG_BOX, &tmB, full_bar(stage), n_tile * BN + 64 * j, kb * WG_PIX, 0);
+                    }
+                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
+                }
+            }
+        } else if (lane == 0) {
             // ------------------------------------------------ TMA producer
             const int slabs = p.is_conv ? (p.Cin / BK) : nk;
             const int tiles_w = p.is_conv ? p.Wo / p.tile_w : 1, tiles_h = p.is_conv ? p.Ho / p.tile_h : 1;
@@ -498,11 +544,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(full_bar(stage), phase);
             const uint32_t a_addr = smem_base + stage * C::STAGE_BYTES;
-            const uint64_t da = make_sw128_desc(a_addr + (uint32_t)wg * (64 * 128)), db = make_sw128_desc(a_addr + C::A_BYTES);
+            // WG: MN-major, warpgroup wg's 64 rows are dY box wg, B spans BN / 64 boxes WG_BOX apart, and a K step of 16
+            // pixel rows is +2048 bytes (+128 in the descriptor's 16-byte units)
+            const uint64_t da = WG ? make_sw128_desc_mn(a_addr + (uint32_t)wg * WG_BOX, WG_BOX)
+                                   : make_sw128_desc(a_addr + (uint32_t)wg * (64 * 128));
+            const uint64_t db = WG ? make_sw128_desc_mn(a_addr + C::A_BYTES, WG_BOX) : make_sw128_desc(a_addr + C::A_BYTES);
             wgmma_fence();
             wgmma_fence_operands(acc);
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) Wgmma<BN, T>::ss(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k));
+            for (int k = 0; k < BK / 16; ++k) {
+                if constexpr (WG) Wgmma<BN, T>::ss_tt(acc, da + (uint64_t)(128 * k), db + (uint64_t)(128 * k));
+                else Wgmma<BN, T>::ss(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k));
+            }
             wgmma_commit();
             wgmma_fence_operands(acc);
             wgmma_wait<1>();                       // the previous k-block's MMAs are done: hand its stage back
@@ -577,11 +630,11 @@ int out_map(CUtensorMap* m, int bf16, const void* base, int n, int M, int batch,
     return encode_map(m, bf16, base, 3, dims, str, box, es, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
-template <int BN, typename T>
+template <int BN, typename T, bool WG = false>
 int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR,
            const GemmParams& p, int64_t work_items, cudaStream_t st) {
     static bool configured = false;
-    auto kern = tc_gemm_kernel<BN, T>;
+    auto kern = tc_gemm_kernel<BN, T, WG>;
     if (!configured) {
         DM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM));
         configured = true;
@@ -651,6 +704,50 @@ __global__ void __launch_bounds__(256) splitk_finish_kernel(const GemmParams p) 
     }
 }
 
+// ---- bias gradient of the weight-gradient mode: db[c] = sum over rows of dy[r, c], without atomics.  Block (cb, k) adds
+// rows k*rows_per_part .. of columns 64cb .. 64cb + 63 in a fixed order (four row lanes, then the lanes in order) into
+// partial row k; bias_grad_finish_kernel adds the partial rows in order.
+template <typename T>
+__global__ void __launch_bounds__(256) bias_grad_partial_kernel(const T* __restrict__ dy, int64_t ld, int64_t rows, int N,
+                                                                int64_t rows_per_part, float* __restrict__ part) {
+    griddep_launch_dependents();
+    griddep_wait();
+    __shared__ float red[4][64];
+    const int cl = threadIdx.x & 63, q = threadIdx.x >> 6, c = blockIdx.x * 64 + cl;
+    const int64_t r0 = (int64_t)blockIdx.y * rows_per_part, r1 = min(rows, r0 + rows_per_part);
+    float s = 0.f;
+    if (c < N)
+        for (int64_t r = r0 + q; r < r1; r += 4) s += Cvt<T>::to_f(dy[r * ld + c]);
+    red[q][cl] = s;
+    __syncthreads();
+    if (q == 0 && c < N) part[(int64_t)blockIdx.y * N + c] = ((red[0][cl] + red[1][cl]) + red[2][cl]) + red[3][cl];
+}
+
+__global__ void __launch_bounds__(256) bias_grad_finish_kernel(const float* __restrict__ part, int parts, int N, float* __restrict__ db) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int c = blockIdx.x * 256 + threadIdx.x;
+    if (c >= N) return;
+    float s = 0.f;
+    for (int k = 0; k < parts; ++k) s += part[(int64_t)k * N + c];
+    db[c] = s;
+}
+
+int bias_grad(int bf16, const void* dy, int64_t ld, int64_t rows, int N, float* db, cudaStream_t st) {
+    int64_t per = dm_ceil_div(rows, 256);                 // at most 256 partial rows, at least 128 dy rows each
+    if (per < 128) per = 128;
+    const int parts = (int)dm_ceil_div(rows, per);
+    float* part = (float*)dm_scratch(DM_SCRATCH_WGRAD, (size_t)parts * N * sizeof(float), st);
+    if (!part) return DM_EDRIVER;
+    const dim3 grid((unsigned)dm_ceil_div(N, 64), (unsigned)parts);
+    if (bf16) DM_CHECK_CUDA(dm_launch(bias_grad_partial_kernel<__nv_bfloat16>, grid, dim3(256), 0, st, (const __nv_bfloat16*)dy, ld, rows, N, per, part));
+    else DM_CHECK_CUDA(dm_launch(bias_grad_partial_kernel<__half>, grid, dim3(256), 0, st, (const __half*)dy, ld, rows, N, per, part));
+    DM_CHECK_LAUNCH();
+    DM_CHECK_CUDA(dm_launch(bias_grad_finish_kernel, dim3((unsigned)dm_ceil_div(N, 256)), dim3(256), 0, st, (const float*)part, parts, N, db));
+    DM_CHECK_LAUNCH();
+    return DM_OK;
+}
+
 struct TileChoice { int bn; int split; };   // split: 0 = let dispatch decide, >= 1 fixed
 
 // Tile width: 64 when there are fewer 128 x 128 tiles than SMs (low-resolution UNet levels) or N <= 64, else 128.  The
@@ -683,7 +780,8 @@ int pick_split(int64_t tiles, int nk, int64_t mn, int N, int act) {
 
 TileChoice choose_tile(int64_t M, int N, int bn_hint) { return {pick_bn(M, N, bn_hint), 0}; }
 
-int dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p_in, const TileChoice& tc, int bf16, cudaStream_t st) {
+int dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p_in, const TileChoice& tc, int bf16, cudaStream_t st,
+             bool wgrad = false) {
     GemmParams p = p_in;
     const int64_t batch = p.batch > 0 ? p.batch : 1;
     const int64_t tiles = dm_ceil_div(p.N, tc.bn) * dm_ceil_div(p.M, BM) * batch;
@@ -706,7 +804,10 @@ int dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p
         }
     }
     const int64_t work = tiles * split;
-    if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half>(tmA, tmB, tmO, tmR, p, work, st);
+    if (wgrad) {
+        if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16, true>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half, true>(tmA, tmB, tmO, tmR, p, work, st);
+        else rc = bf16 ? launch<128, __nv_bfloat16, true>(tmA, tmB, tmO, tmR, p, work, st) : launch<128, __half, true>(tmA, tmB, tmO, tmR, p, work, st);
+    } else if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half>(tmA, tmB, tmO, tmR, p, work, st);
     else rc = bf16 ? launch<128, __nv_bfloat16>(tmA, tmB, tmO, tmR, p, work, st) : launch<128, __half>(tmA, tmB, tmO, tmR, p, work, st);
     if (rc || split <= 1) return rc;
     const int64_t n4 = batch * p.M * (p.N >> 2);
@@ -730,6 +831,16 @@ void fill_epilogue(GemmParams& p, const dm_epilogue* e, int N) {
     p.out_scale = e ? e->out_scale : 1.0f;
     p.act = e ? e->act : 0;
     p.out_f32 = e ? e->out_f32 : 0;
+}
+
+// Weight gradient: p holds the GEMM view [M' = Cout, N', K' = 64 * pixel blocks] and the operand geometry; dW [M', N'] is
+// written in fp32 (overwritten, row pitch N').  Planned by the forward's choose_tile / pick_split, so dm_gemm_plan(M', N',
+// K') reports the tile and split this call uses; a split goes through the workspace slices and splitk_finish_kernel.
+int wgrad_run(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, int bf16, float* dw, cudaStream_t st) {
+    p.batch = 1;
+    p.out = dw; p.ldc = p.N; p.out_f32 = 1;
+    p.alpha = 1.0f; p.out_scale = 1.0f; p.rows_per_vec = 1;
+    return dispatch(tmA, tmB, p, choose_tile(p.M, p.N, 0), bf16, st, true);
 }
 
 }  // namespace
@@ -838,6 +949,95 @@ extern "C" int dm_conv2d(int bf16, const void* x, int n_img, int H, int W, int C
     p.out = y; p.ldc = (int)ldc; p.out_batch_stride = 0;
     fill_epilogue(p, ep, Cout);
     return dispatch(tmA, tmB, p, tc, bf16, (cudaStream_t)stream);
+}
+
+static int wgrad_storage_check(int bf16, const char* name) {
+    if (bf16 == 2) {
+        dm_set_error("%s: weight gradients in fp32 storage (high-precision mode) are not implemented", name);
+        return DM_EUNSUPPORTED;
+    }
+    DM_REQUIRE(bf16 == 0 || bf16 == 1, "storage selector: 0 fp16, 1 bf16");
+    return DM_OK;
+}
+
+extern "C" int dm_conv2d_wgrad(int bf16, const void* x, int n_img, int H, int W, int Cin, const void* dy, int64_t ld_dy,
+                               int Cout, int ksize, int stride, int pad_t, int pad_l, int Ho, int Wo, float* dw, float* db,
+                               void* stream) {
+    if (int rc = wgrad_storage_check(bf16, "dm_conv2d_wgrad")) return rc;
+    DM_REQUIRE(x && dy && dw, "null pointer");
+    DM_REQUIRE((((uintptr_t)x | (uintptr_t)dy | (uintptr_t)dw) & 15) == 0 && ((uintptr_t)db & 3) == 0,
+               "x, dy and dw 16-byte aligned, db 4-byte aligned");
+    DM_REQUIRE(n_img > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Cout > 0, "positive extents");
+    DM_REQUIRE(Cin > 0 && Cin % BK == 0, "Cin must be a multiple of 64 (pad the channels)");
+    DM_REQUIRE(ksize == 3 || ksize == 1, "3x3 or 1x1");
+    DM_REQUIRE(stride == 1 || stride == 2, "stride 1 or 2");
+    DM_REQUIRE(pad_t >= 0 && pad_l >= 0, "non-negative padding");
+    DM_REQUIRE(ld_dy % 8 == 0 && ld_dy >= Cout, "dy pixel stride: a multiple of 8 elements (16 bytes), at least Cout");
+    // the forward's tiling rule at 64 pixels: a K-block is one box {tile_w, tile_h, tile_n} of output pixels; images past
+    // n_img are zero-filled, so the pixel count need not be a multiple of 64
+    const int tile_w = Wo < WG_PIX ? Wo : WG_PIX;
+    const int tile_h = (WG_PIX / tile_w) < Ho ? (WG_PIX / tile_w) : Ho;
+    const int tile_n = WG_PIX / (tile_w * tile_h);
+    DM_REQUIRE(tile_w * tile_h * tile_n == WG_PIX && Wo % tile_w == 0 && Ho % tile_h == 0,
+               "output extent must tile into 64-pixel boxes (power-of-two sizes)");
+    const int64_t nk = (int64_t)(Wo / tile_w) * (Ho / tile_h) * dm_ceil_div(n_img, tile_n);
+    DM_REQUIRE(nk * WG_PIX < (1ll << 31), "at most 2^31 output pixels");
+    const int taps = ksize * ksize;
+    CUtensorMap tmA, tmB;
+    {
+        // dY [n, Ho, Wo, ld_dy], first Cout channels: boxes {64 channels, tile_w, tile_h, tile_n}
+        uint64_t dims[4] = {(uint64_t)Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)n_img};
+        uint64_t str[3] = {(uint64_t)ld_dy * 2, (uint64_t)Wo * ld_dy * 2, (uint64_t)Ho * Wo * ld_dy * 2};
+        uint32_t box[4] = {64, (uint32_t)tile_w, (uint32_t)tile_h, (uint32_t)tile_n}, es[4] = {1, 1, 1, 1};
+        int rc = encode_map(&tmA, bf16, dy, 4, dims, str, box, es); if (rc) return rc;
+    }
+    {
+        // x through the forward's map: the same pixels at a tap's shifted origin, element strides for stride 2
+        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)n_img};
+        uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
+        uint32_t box[4] = {64, (uint32_t)(tile_w * stride), (uint32_t)(tile_h * stride), (uint32_t)tile_n};
+        uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
+        int rc = encode_map(&tmB, bf16, x, 4, dims, str, box, es); if (rc) return rc;
+    }
+    GemmParams p; memset(&p, 0, sizeof(p));
+    p.M = Cout; p.N = taps * Cin; p.K = (int)(nk * WG_PIX);
+    p.is_conv = 1; p.Cin = Cin; p.taps = taps; p.kw_n = ksize;
+    p.Ho = Ho; p.Wo = Wo; p.tile_w = tile_w; p.tile_h = tile_h; p.tile_n = tile_n; p.stride = stride; p.pad_t = pad_t; p.pad_l = pad_l;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = wgrad_run(tmA, tmB, p, bf16, dw, st);
+    if (rc || !db) return rc;
+    return bias_grad(bf16, dy, ld_dy, (int64_t)n_img * Ho * Wo, Cout, db, st);
+}
+
+extern "C" int dm_gemm_wgrad(int bf16, const void* dy, int64_t ld_dy, const void* x, int64_t ldx, int M, int N, int K,
+                             float* dw, float* db, void* stream) {
+    if (int rc = wgrad_storage_check(bf16, "dm_gemm_wgrad")) return rc;
+    DM_REQUIRE(dy && x && dw, "null pointer");
+    DM_REQUIRE((((uintptr_t)x | (uintptr_t)dy | (uintptr_t)dw) & 15) == 0 && ((uintptr_t)db & 3) == 0,
+               "x, dy and dw 16-byte aligned, db 4-byte aligned");
+    DM_REQUIRE(M > 0 && M <= (1 << 30) && N > 0 && K > 0 && K % BK == 0, "1 <= M <= 2^30, N >= 1, K a positive multiple of 64");
+    DM_REQUIRE(ld_dy % 8 == 0 && ldx % 8 == 0 && ld_dy >= N && ldx >= K,
+               "row strides: multiples of 8 elements (16 bytes), at least N (dy) and K (x)");
+    CUtensorMap tmA, tmB;
+    {
+        // dY [M, ld_dy] and x [M, ldx] token-major: boxes of 64 columns x 64 rows, rows past M zero-filled
+        uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, 1};
+        uint64_t str[2] = {(uint64_t)ld_dy * 2, (uint64_t)M * ld_dy * 2};
+        uint32_t box[3] = {64, WG_PIX, 1}, es[3] = {1, 1, 1};
+        int rc = encode_map(&tmA, bf16, dy, 3, dims, str, box, es); if (rc) return rc;
+    }
+    {
+        uint64_t dims[3] = {(uint64_t)K, (uint64_t)M, 1};
+        uint64_t str[2] = {(uint64_t)ldx * 2, (uint64_t)M * ldx * 2};
+        uint32_t box[3] = {64, WG_PIX, 1}, es[3] = {1, 1, 1};
+        int rc = encode_map(&tmB, bf16, x, 3, dims, str, box, es); if (rc) return rc;
+    }
+    GemmParams p; memset(&p, 0, sizeof(p));
+    p.M = N; p.N = K; p.K = (int)dm_ceil_div(M, WG_PIX) * WG_PIX;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = wgrad_run(tmA, tmB, p, bf16, dw, st);
+    if (rc || !db) return rc;
+    return bias_grad(bf16, dy, ld_dy, M, N, db, st);
 }
 
 

@@ -171,6 +171,15 @@ def ptr_any(t):
     return C.c_void_p(t.data_ptr())
 
 
+def _conv_out_hw(H, W, ksize, stride, pad, out_hw):
+    """output extent of conv2d: symmetric padding pad = (top, left) unless out_hw fixes it (then the bottom / right
+    padding is whatever out_hw implies)"""
+    if out_hw is not None:
+        return tuple(out_hw)
+    pt, pl = pad
+    return (H + 2 * pt - ksize) // stride + 1, (W + 2 * pl - ksize) // stride + 1
+
+
 def conv2d(x, w, ksize, stride=1, pad=(1, 1), out_hw=None, bias=None, rowvec=None, residual=None, out_scale=1.0,
            act=None, out=None, out_f32=False, bn=0):
     """x [n,H,W,Cin] NHWC (contiguous), w [Cout, k*k*Cin] -> y [n,Ho,Wo,Cout] (or into `out`, whose last-dim
@@ -181,12 +190,7 @@ def conv2d(x, w, ksize, stride=1, pad=(1, 1), out_hw=None, bias=None, rowvec=Non
     n, H, W, Cin = x.shape
     Cout = w.shape[0]
     assert w.shape[1] == ksize * ksize * Cin
-    if out_hw is None:
-        pt, pl = pad
-        Ho = (H + 2 * pt - ksize) // stride + 1
-        Wo = (W + 2 * pl - ksize) // stride + 1
-    else:
-        Ho, Wo = out_hw
+    Ho, Wo = _conv_out_hw(H, W, ksize, stride, pad, out_hw)
     if out is None:
         out = torch.empty(n, Ho, Wo, Cout, device=x.device, dtype=torch.float32 if out_f32 else x.dtype)
     assert out.stride(-1) == 1 and out.shape[:3] == (n, Ho, Wo)
@@ -202,6 +206,51 @@ def conv2d(x, w, ksize, stride=1, pad=(1, 1), out_hw=None, bias=None, rowvec=Non
     check(lib().dm_conv2d(bf, ptr_any(x), n, H, W, Cin, ptr_any(w), Cout, ksize, stride, pad[0], pad[1], Ho, Wo,
                           ptr_any(out), ldc, C.byref(e), bn, stream_ptr()), "dm_conv2d")
     return out
+
+
+def _wgrad_storage(t):
+    bf = _is_bf16(t)
+    if bf == 2:
+        raise TypeError("weight gradients need fp16 / bf16 storage (the fp32 high-precision mode has none)")
+    return bf
+
+
+def conv2d_wgrad(x, dy, ksize, stride=1, pad=(1, 1), out_hw=None, bias=False):
+    """Weight (and bias) gradient of conv2d(x, w, ksize, stride, pad, out_hw) for the output gradient dy [n,Ho,Wo,Cout],
+    which may be a channel slice of a wider buffer (its pixel stride is passed on).  Returns (dw, db): dw [Cout, k*k*Cin]
+    fp32 in conv2d's weight layout (tap-major, channel-minor, padded channels included), db [Cout] fp32 or None."""
+    _ensure_workspace()
+    bf = _wgrad_storage(x)
+    assert dy.dtype == x.dtype and x.is_contiguous()
+    n, H, W, Cin = x.shape
+    Ho, Wo = _conv_out_hw(H, W, ksize, stride, pad, out_hw)
+    assert dy.shape[:3] == (n, Ho, Wo) and dy.stride(-1) == 1
+    ld = dy.stride(2)
+    assert dy.stride(1) == Wo * ld and dy.stride(0) == Ho * Wo * ld
+    Cout = dy.shape[3]
+    dw = torch.empty(Cout, ksize * ksize * Cin, device=x.device, dtype=torch.float32)
+    db = torch.empty(Cout, device=x.device, dtype=torch.float32) if bias else None
+    check(lib().dm_conv2d_wgrad(bf, ptr_any(x), n, H, W, Cin, ptr_any(dy), ld, Cout, ksize, stride, pad[0], pad[1], Ho, Wo,
+                                ptr_any(dw), ptr_any(db) if bias else None, stream_ptr()), "dm_conv2d_wgrad")
+    return dw, db
+
+
+def gemm_wgrad(dy, x, bias=False):
+    """Weight (and bias) gradient of gemm(x, w) = x w^T for the output gradient dy: dy [.., M, N], x [.., M, K] (leading
+    dims fold into M; row strides allowed, e.g. a column slice of a fused projection).  Returns (dw, db): dw [N, K] fp32 in
+    the layout and row order of w, db [N] fp32 or None."""
+    _ensure_workspace()
+    bf = _wgrad_storage(x)
+    assert dy.dtype == x.dtype and dy.stride(-1) == 1 and x.stride(-1) == 1
+    dy2, x2 = _hp_rows(dy), _hp_rows(x)
+    M, N = dy2.shape
+    K = x2.shape[1]
+    assert x2.shape[0] == M
+    dw = torch.empty(N, K, device=x.device, dtype=torch.float32)
+    db = torch.empty(N, device=x.device, dtype=torch.float32) if bias else None
+    check(lib().dm_gemm_wgrad(bf, ptr_any(dy2), dy2.stride(0), ptr_any(x2), x2.stride(0), M, N, K, ptr_any(dw),
+                              ptr_any(db) if bias else None, stream_ptr()), "dm_gemm_wgrad")
+    return dw, db
 
 
 class Csd(C.Structure):

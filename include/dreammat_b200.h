@@ -15,7 +15,10 @@
  *
  * DETERMINISM: with the same inputs the training step's gradient path returns bit-identical results (no fp32 atomic decides
  * a summation order).  Still accumulated with fp32 atomics: the logged sums (norms of dm_conv2d_csd / dm_sds_grad, reg_sums
- * of the shading) and the adjoint of dm_resize_bilinear (renders that are not 512^2).  dm_groupnorm / dm_groupnorm_bwd (per-block partial sums), dm_antialias_fwd / _bwd (per-pixel pair buckets) and
+ * of the shading) and the adjoint of dm_resize_bilinear (renders that are not 512^2).  Weight gradients (dm_conv2d_wgrad /
+ * dm_gemm_wgrad) sum each element in one fixed K order, split-K slices in slice order, and the bias gradient's per-block
+ * partial rows in row order.  dm_groupnorm / dm_groupnorm_bwd (per-block partial sums), the bias gradient of
+ * dm_conv2d_wgrad / dm_gemm_wgrad (per-block partial rows), dm_antialias_fwd / _bwd (per-pixel pair buckets) and
  * dm_hashgrid_mlp_bwd (int64 fixed-point grid gradient) need scratch for that which their signatures have no room for; the library allocates it once per device, on
  * the first call (not while the stream is being captured: run a call once before capturing it), and never frees it.  Calls
  * on one device must not run concurrently on two streams.
@@ -230,6 +233,22 @@ int dm_gemm(int bf16, const void* A, int64_t lda, int64_t a_batch_stride, const 
 int dm_conv2d(int bf16, const void* x, int n_img, int H, int W, int Cin, const void* w, int Cout, int ksize,
               int stride, int pad_t, int pad_l, int Ho, int Wo, void* y, int64_t ldc, const dm_epilogue* ep,
               int bn_hint, void* stream);
+/* Weight gradients (the `weight.grad` / `bias.grad` autograd computes for a conv / linear layer).  The tensor-core kernel
+ * reduces over the pixel / token axis straight from the NHWC / token-major buffers (no transpose, no im2col); the pixel
+ * or token count need not be a multiple of 64.  Planned as the GEMM view [M' = Cout (N), N' = k*k*Cin (K), K' = pixels
+ * (M) rounded up to 64], so dm_gemm_plan(M', N', K', 0, 0, ...) reports the tile and split-K a call uses.  dW is written
+ * in exactly the layout of the weight the forward consumed, so it can update that weight in place.  16-bit storage only:
+ * bf16 == 2 (fp32 storage) returns DM_EUNSUPPORTED.  Bad shapes, strides or alignment return DM_EINVAL before any launch.
+ *
+ * dW[Cout, k*k*Cin] (fp32, overwritten) = d/dw of dm_conv2d(x, w, ...) . dy; db[Cout] (fp32, may be NULL) = sum_p dy.
+ * x [n,H,W,Cin] (Cin % 64 == 0), dy [n,Ho,Wo,ld_dy] (first Cout channels; ld_dy % 8 == 0), same ksize / stride /
+ * pad_t / pad_l / Ho / Wo conventions as dm_conv2d.  Deterministic. */
+int dm_conv2d_wgrad(int bf16, const void* x, int n_img, int H, int W, int Cin, const void* dy, int64_t ld_dy, int Cout,
+                    int ksize, int stride, int pad_t, int pad_l, int Ho, int Wo, float* dw, float* db, void* stream);
+/* dW[N, K] (fp32, overwritten) = sum_m dy[m, :]^T x[m, :]; db[N] = sum_m dy[m, :] (may be NULL).  dy [M, ld_dy],
+ * x [M, ldx]; K % 64 == 0; M arbitrary (>= 1).  Deterministic. */
+int dm_gemm_wgrad(int bf16, const void* dy, int64_t ld_dy, const void* x, int64_t ldx, int M, int N, int K, float* dw,
+                  float* db, void* stream);
 
 /* conv_out of the UNet with the CSD / SDS combination fused into its epilogue: the model-level tail of
  * `dm_unet_fwd_sds` (SURVEY.md section 8b).  Replaces conv_out (dreammat_guidance.py:274-282), the `.sample` layout /
