@@ -78,6 +78,9 @@ SIGNATURES = {
     "dm_groupnorm_bwd": (C.c_int, [C.c_int, P, P] + [C.c_int] * 4 + [P, P, F, C.c_int, P, P, P, P, P]),
     "dm_layernorm": (C.c_int, [C.c_int, P, I64, C.c_int, P, P, F, P, P]),
     "dm_geglu": (C.c_int, [C.c_int, P, I64, C.c_int, P, P]),
+    "dm_layernorm_bwd": (C.c_int, [C.c_int, P, P, I64, C.c_int, P, F, P, P, P, P, P]),
+    "dm_groupnorm_affine_grad": (C.c_int, [C.c_int, P, P] + [C.c_int] * 4 + [P, P, C.c_int, P, P, P, P]),
+    "dm_geglu_bwd": (C.c_int, [C.c_int, P, P, I64, C.c_int, P, P]),
     "dm_upsample2x": (C.c_int, [C.c_int, P] + [C.c_int] * 5 + [P, P]),
     "dm_axpby2d": (C.c_int, [C.c_int, P, I64, F, P, I64, F, I64, C.c_int, P, I64, P]),
     "dm_transpose": (C.c_int, [C.c_int, P, C.c_int, C.c_int, C.c_int, I64, I64, P, I64, I64, P]),
@@ -92,6 +95,9 @@ SIGNATURES = {
     "dm_timestep_embedding": (C.c_int, [C.c_int, P, C.c_int, C.c_int, P, P]),
     "dm_silu": (C.c_int, [C.c_int, P, I64, P, P]),
     "dm_attention": (C.c_int, [C.c_int, P, I64, I64, P, P, I64, I64, P, I64, I64] + [C.c_int] * 5 + [F, P]),
+    "dm_attention_lse": (C.c_int, [C.c_int, P, I64, I64, P, P, I64, I64, P, I64, I64] + [C.c_int] * 5 + [F, P, P]),
+    "dm_attention_bwd": (C.c_int, [C.c_int, P, I64, I64, P, P, I64, I64, P, I64, I64, P, I64, I64, P, P, I64, I64, P, I64,
+                                   I64, P, I64, I64, P] + [C.c_int] * 5 + [F, P]),
     "dm_cond_gather": (C.c_int, [C.c_int, P, P, P, C.c_int, I64, P, P, C.c_int, C.c_int, P, P]),
     "dm_envlight_latlong_to_cube": (C.c_int, [P, C.c_int, C.c_int, F, C.c_int, P, P]),
     "dm_envlight_downsample": (C.c_int, [P, C.c_int, P, P]),

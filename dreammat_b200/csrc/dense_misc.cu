@@ -1,5 +1,6 @@
 // dense_misc.cu -- the non-GEMM kernels of the VAE-encoder / UNet / ControlNet path (rows a7, a8):
-// GroupNorm(+SiLU) forward/backward, LayerNorm, GEGLU, nearest 2x upsample, strided copies,
+// GroupNorm(+SiLU) forward/backward, LayerNorm, GEGLU and their backward (with the norms' affine gradients), nearest 2x
+// upsample, strided copies,
 // transposes, row softmax forward/backward, layout / dtype conversion at the fp32 boundaries,
 // posterior sampling, add_noise and the sinusoidal timestep embedding.
 // NHWC activations, fp16 or bf16 storage, fp32 math.  All are HBM-bound streaming kernels:
@@ -707,6 +708,165 @@ __global__ void __launch_bounds__(256) silu_kernel(const T* __restrict__ x, int6
         y[i] = H<T>::t(silu_f(H<T>::f(x[i])));
 }
 
+// ----------------------------------------------------------------------------------- norm / GEGLU backward
+// LayerNorm backward, warp per row (the forward's mapping): mean / rstd recomputed from x with the forward's arithmetic,
+// g = dy * gamma, dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dx_add).  (mean, rstd) of each row go to `rstats`
+// for the affine-gradient kernel.
+template <typename T>
+__global__ void __launch_bounds__(256) layernorm_bwd_kernel(const T* __restrict__ x, const T* __restrict__ dy, int64_t M,
+                                                            int C, const T* __restrict__ gamma, float eps,
+                                                            const T* __restrict__ dx_add, T* __restrict__ dx,
+                                                            float* __restrict__ rstats) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= M) return;
+    const int lane = threadIdx.x & 31, nv = C >> 3;
+    const T* xr = x + row * C;
+    float vals[40], g[40];
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        const int v = lane + 32 * k;
+        if (v < nv) {
+            uint4 u = *reinterpret_cast<const uint4*>(xr + 8 * v);
+            uint4 ud = *reinterpret_cast<const uint4*>(dy + row * C + 8 * v);
+            uint4 ug = *reinterpret_cast<const uint4*>(gamma + 8 * v);
+            const T* h = reinterpret_cast<const T*>(&u); const T* hd = reinterpret_cast<const T*>(&ud);
+            const T* hg = reinterpret_cast<const T*>(&ug);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                float f = H<T>::f(h[j]); vals[8 * k + j] = f; s += f;
+                g[8 * k + j] = H<T>::f(hd[j]) * H<T>::f(hg[j]);
+            }
+        }
+    }
+    s = warp_sum(s);
+    const float mean = s / (float)C;
+    float ss = 0.f;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        if (lane + 32 * k < nv) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { float d = vals[8 * k + j] - mean; ss += d * d; }
+        }
+    }
+    ss = warp_sum(ss);
+    const float rstd = rsqrtf(ss / (float)C + eps);
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        if (lane + 32 * k < nv) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                vals[8 * k + j] = (vals[8 * k + j] - mean) * rstd;     // xhat
+                s1 += g[8 * k + j];
+                s2 = fmaf(g[8 * k + j], vals[8 * k + j], s2);
+            }
+        }
+    }
+    s1 = warp_sum(s1) / (float)C;
+    s2 = warp_sum(s2) / (float)C;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        const int v = lane + 32 * k;
+        if (v < nv) {
+            uint4 ua = dx_add ? *reinterpret_cast<const uint4*>(dx_add + row * C + 8 * v) : make_uint4(0, 0, 0, 0);
+            const T* ha = reinterpret_cast<const T*>(&ua);
+            uint4 o; T* oh = reinterpret_cast<T*>(&o);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                float val = rstd * (g[8 * k + j] - s1 - vals[8 * k + j] * s2);
+                if (dx_add) val += H<T>::f(ha[j]);
+                oh[j] = H<T>::t(val);
+            }
+            *reinterpret_cast<uint4*>(dx + row * C + 8 * v) = o;
+        }
+    }
+    if (lane == 0) { rstats[2 * row] = mean; rstats[2 * row + 1] = rstd; }
+}
+
+// Affine-parameter gradients of LayerNorm (G == 0: stats per row) and GroupNorm (stats per (image, group), HW rows per
+// image, optional SiLU after the affine): a thread owns one 8-channel vector and the rows [chunk*rpc, +rpc) and writes its
+// sums to its own slots of the chunk's partial row part[chunk][2C] = (sum dy' xhat | sum dy'); affine_finish_kernel adds
+// the chunks' rows in chunk order, so the result is bit-identical from run to run.
+template <typename T>
+__global__ void __launch_bounds__(128) affine_partials_kernel(const T* __restrict__ x, const T* __restrict__ dz, int64_t rows,
+                                                              int C, int HW, int G, const float* __restrict__ stats,
+                                                              const T* __restrict__ gamma, const T* __restrict__ beta,
+                                                              int silu, int rpc, float* __restrict__ part) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int v = blockIdx.y * blockDim.x + threadIdx.x;
+    if (v >= C / 8) return;
+    const int64_t r0 = (int64_t)blockIdx.x * rpc, r1 = min(rows, r0 + rpc);
+    float gm[8], bt[8], dg[8] = {}, db[8] = {};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        gm[k] = silu ? H<T>::f(gamma[8 * v + k]) : 0.f;
+        bt[k] = silu ? H<T>::f(beta[8 * v + k]) : 0.f;
+    }
+    const int cpg = G ? C / G : 1;
+    for (int64_t r = r0; r < r1; ++r) {
+        uint4 ux = *reinterpret_cast<const uint4*>(x + r * C + 8 * v), ud = *reinterpret_cast<const uint4*>(dz + r * C + 8 * v);
+        const T* hx = reinterpret_cast<const T*>(&ux); const T* hd = reinterpret_cast<const T*>(&ud);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int64_t si = G ? (r / HW * G + (8 * v + k) / cpg) * 2 : 2 * r;
+            const float xhat = (H<T>::f(hx[k]) - stats[si]) * stats[si + 1];
+            float d = H<T>::f(hd[k]);
+            if (silu) d *= silu_grad(fmaf(xhat, gm[k], bt[k]));
+            dg[k] = fmaf(d, xhat, dg[k]);
+            db[k] += d;
+        }
+    }
+    float* pr = part + (int64_t)blockIdx.x * 2 * C + 8 * v;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { pr[k] = dg[k]; pr[C + k] = db[k]; }
+}
+
+__global__ void __launch_bounds__(256) affine_finish_kernel(const float* __restrict__ part, int chunks, int C,
+                                                            float* __restrict__ dgamma, float* __restrict__ dbeta) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= 2 * C) return;
+    float s = 0.f;
+    for (int c = 0; c < chunks; ++c) s += part[(int64_t)c * 2 * C + j];
+    if (j < C) dgamma[j] = s; else dbeta[j - C] = s;
+}
+
+// GEGLU backward on the interleaved pre-activation of the fused GEGLU epilogue: h [M, 2D] in blocks of 64 columns (32 value
+// columns, then their 32 gate columns), out[m, 32b + r] = h[m, 64b + r] * gelu(h[m, 64b + 32 + r]) (erf GELU).
+//   dh[value] = dout * gelu(gate),  dh[gate] = dout * value * gelu'(gate),  gelu'(g) = Phi(g) + g phi(g)
+template <typename T>
+__global__ void __launch_bounds__(256) geglu_bwd_kernel(const T* __restrict__ h, const T* __restrict__ dout, int64_t M, int D,
+                                                        T* __restrict__ dh) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int64_t n = M * (int64_t)(D / 8);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t m = i / (D / 8);
+        const int j = (int)(i - m * (D / 8)) * 8;                  // output column (8 of them)
+        const int64_t hv = m * 2 * D + 64 * (j / 32) + j % 32;    // their value columns; gate columns at + 32
+        uint4 a = *reinterpret_cast<const uint4*>(h + hv), g = *reinterpret_cast<const uint4*>(h + hv + 32);
+        uint4 d = *reinterpret_cast<const uint4*>(dout + m * D + j);
+        const T* ha = reinterpret_cast<const T*>(&a); const T* hg = reinterpret_cast<const T*>(&g);
+        const T* hd = reinterpret_cast<const T*>(&d);
+        uint4 ov, og; T* pv = reinterpret_cast<T*>(&ov); T* pg = reinterpret_cast<T*>(&og);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const float gv = H<T>::f(hg[k]), dv = H<T>::f(hd[k]);
+            const float cdf = 0.5f * (1.0f + erff(gv * 0.70710678118654752f));
+            const float pdf = 0.3989422804014327f * expf(-0.5f * gv * gv);
+            pv[k] = H<T>::t(dv * gv * cdf);
+            pg[k] = H<T>::t(dv * H<T>::f(ha[k]) * (cdf + gv * pdf));
+        }
+        *reinterpret_cast<uint4*>(dh + hv) = ov;
+        *reinterpret_cast<uint4*>(dh + hv + 32) = og;
+    }
+}
+
 inline int grid_for(int64_t work, int threads = 256) {
     int64_t b = dm_ceil_div(work, threads);
     int64_t cap = (int64_t)DM_NUM_SMS * 8;
@@ -939,6 +1099,71 @@ extern "C" int dm_silu(int bf16, const void* x, int64_t n, void* y, void* stream
     DM_DTYPE_OK(bf16);
     DM_REQUIRE(x && y, "null pointer");
     DM_DISPATCH_T3(bf16, silu_kernel<T><<<grid_for(n), 256, 0, (cudaStream_t)stream>>>((const T*)x, n, (T*)y));
+    DM_CHECK_LAUNCH();
+    return DM_OK;
+}
+
+// partial rows of the affine gradients (and LayerNorm's per-row stats) in the library scratch; rows per chunk chosen so
+// that there are about 4 CTAs per SM
+static int affine_grad(int bf16, const void* x, const void* dz, int64_t rows, int C, int HW, int G, const float* stats,
+                       const void* gamma, const void* beta, int silu, float* part, float* dgamma, float* dbeta,
+                       cudaStream_t st) {
+    const int rpc = (int)(rows / (DM_NUM_SMS * 4)) + 1 < 16 ? 16 : (int)(rows / (DM_NUM_SMS * 4)) + 1;
+    const int chunks = (int)dm_ceil_div(rows, rpc);
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(affine_partials_kernel<T>, dim3((unsigned)chunks, (unsigned)dm_ceil_div(C / 8, 128)),
+                                                dim3(128), 0, st, (const T*)x, (const T*)dz, rows, C, HW, G, stats,
+                                                (const T*)gamma, (const T*)beta, silu, rpc, part)));
+    DM_CHECK_LAUNCH();
+    DM_CHECK_CUDA(dm_launch(affine_finish_kernel, dim3((unsigned)dm_ceil_div(2 * C, 256)), dim3(256), 0, st, (const float*)part,
+                            chunks, C, dgamma, dbeta));
+    DM_CHECK_LAUNCH();
+    return DM_OK;
+}
+static size_t affine_part_bytes(int64_t rows, int C) {
+    const int rpc = (int)(rows / (DM_NUM_SMS * 4)) + 1 < 16 ? 16 : (int)(rows / (DM_NUM_SMS * 4)) + 1;
+    return (size_t)dm_ceil_div(rows, rpc) * 2 * C * sizeof(float);
+}
+
+extern "C" int dm_layernorm_bwd(int bf16, const void* x, const void* dy, int64_t M, int C, const void* gamma, float eps,
+                                const void* dx_add, void* dx, float* dgamma, float* dbeta, void* stream) {
+    DM_DTYPE_OK(bf16);
+    if (bf16 == 2) { dm_set_error("dm_layernorm_bwd: fp32 storage is not supported (16-bit only)"); return DM_EUNSUPPORTED; }
+    DM_REQUIRE(x && dy && gamma && dx && dgamma && dbeta, "null pointer");
+    DM_REQUIRE(C <= 1280 && C % 8 == 0 && M > 0, "C <= 1280, multiple of 8; M >= 1");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t pb = affine_part_bytes(M, C);
+    float* part = (float*)dm_scratch(DM_SCRATCH_AFFINE, pb + (size_t)M * 2 * sizeof(float), st);
+    if (!part) return DM_EDRIVER;
+    float* rstats = part + pb / sizeof(float);
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(layernorm_bwd_kernel<T>, dim3((unsigned)dm_ceil_div(M, 8)), dim3(256), 0, st,
+                                                (const T*)x, (const T*)dy, M, C, (const T*)gamma, eps, (const T*)dx_add,
+                                                (T*)dx, rstats)));
+    DM_CHECK_LAUNCH();
+    return affine_grad(bf16, x, dy, M, C, 1, 0, rstats, gamma, gamma, 0, part, dgamma, dbeta, st);
+}
+
+extern "C" int dm_groupnorm_affine_grad(int bf16, const void* x, const void* dz, int n_img, int HW, int C, int G,
+                                        const void* gamma, const void* beta, int silu, const float* stats, float* dgamma,
+                                        float* dbeta, void* stream) {
+    DM_DTYPE_OK(bf16);
+    if (bf16 == 2) { dm_set_error("dm_groupnorm_affine_grad: fp32 storage is not supported (16-bit only)"); return DM_EUNSUPPORTED; }
+    DM_REQUIRE(x && dz && stats && dgamma && dbeta && (!silu || (gamma && beta)), "null pointer");
+    DM_REQUIRE(C % 8 == 0 && G > 0 && C % G == 0 && n_img > 0 && HW > 0, "channel layout");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t rows = (int64_t)n_img * HW;
+    float* part = (float*)dm_scratch(DM_SCRATCH_AFFINE, affine_part_bytes(rows, C), st);
+    if (!part) return DM_EDRIVER;
+    return affine_grad(bf16, x, dz, rows, C, HW, G, stats, gamma, beta, silu, part, dgamma, dbeta, st);
+}
+
+extern "C" int dm_geglu_bwd(int bf16, const void* h, const void* dout, int64_t M, int D, void* dh, void* stream) {
+    DM_DTYPE_OK(bf16);
+    if (bf16 == 2) { dm_set_error("dm_geglu_bwd: fp32 storage is not supported (16-bit only)"); return DM_EUNSUPPORTED; }
+    DM_REQUIRE(h && dout && dh, "null pointer");
+    DM_REQUIRE(D % 32 == 0 && M >= 0, "D multiple of 32 (interleaved 32-column value / gate blocks)");
+    if (M == 0) return DM_OK;
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(geglu_bwd_kernel<T>, dim3((unsigned)grid_for(M * (D / 8))), dim3(256), 0,
+                                                (cudaStream_t)stream, (const T*)h, (const T*)dout, M, D, (T*)dh)));
     DM_CHECK_LAUNCH();
     return DM_OK;
 }

@@ -333,6 +333,36 @@ def layernorm(x, gamma, beta, eps=1e-5):
     return y
 
 
+def layernorm_bwd(x, dy, gamma, eps=1e-5, dx_add=None):
+    """Backward of layernorm(x, gamma, beta, eps): returns (dx [storage dtype] (+ dx_add), dgamma, dbeta [C] fp32).
+    16-bit storage only; deterministic."""
+    bf = _is_bf16(x)
+    assert x.is_contiguous() and dy.is_contiguous() and dy.shape == x.shape
+    assert dx_add is None or (dx_add.is_contiguous() and dx_add.shape == x.shape)
+    Cc = x.shape[-1]
+    dx = torch.empty_like(x)
+    dg = torch.empty(Cc, device=x.device, dtype=torch.float32)
+    db = torch.empty(Cc, device=x.device, dtype=torch.float32)
+    check(lib().dm_layernorm_bwd(bf, ptr_any(x), ptr_any(dy), x.numel() // Cc, Cc, ptr_any(gamma), eps,
+                                 ptr_any(dx_add) if dx_add is not None else None, ptr_any(dx), ptr_any(dg), ptr_any(db),
+                                 stream_ptr()), "dm_layernorm_bwd")
+    return dx, dg, db
+
+
+def groupnorm_affine_grad(x, dz, gamma, beta, stats, groups=32, silu=False):
+    """(dgamma, dbeta) [C] fp32 of groupnorm(x, gamma, beta, groups, silu=silu) for the output gradient dz (x, dz dense
+    [n, H, W, C]; stats from groupnorm).  16-bit storage only; deterministic."""
+    bf = _is_bf16(x)
+    n, Hh, W, Cc = x.shape
+    assert x.is_contiguous() and dz.is_contiguous() and dz.shape == x.shape
+    dg = torch.empty(Cc, device=x.device, dtype=torch.float32)
+    db = torch.empty(Cc, device=x.device, dtype=torch.float32)
+    check(lib().dm_groupnorm_affine_grad(bf, ptr_any(x), ptr_any(dz), n, Hh * W, Cc, groups, ptr_any(gamma), ptr_any(beta),
+                                         1 if silu else 0, ptr_any(stats), ptr_any(dg), ptr_any(db), stream_ptr()),
+          "dm_groupnorm_affine_grad")
+    return dg, db
+
+
 def geglu_interleave(w):
     """Row order the fused GEGLU epilogue of dm_gemm expects: [value | gate] halves (diffusers GEGLU.proj,
     attention.py chunk(2, dim=-1)) -> alternating blocks of 32 value rows and their 32 gate rows."""
@@ -350,6 +380,19 @@ def geglu(h):
     out = torch.empty(*h.shape[:-1], D, device=h.device, dtype=h.dtype)
     check(lib().dm_geglu(bf, ptr_any(h), M, D, ptr_any(out), stream_ptr()), "dm_geglu")
     return out
+
+
+def geglu_bwd(h, dout):
+    """Gradient of the fused GEGLU epilogue (gemm(..., act="geglu")) with respect to its interleaved pre-activation h
+    [.., 2D] (geglu_interleave's row order) for dout [.., D]: dh in h's layout.  16-bit storage only."""
+    bf = _is_bf16(h)
+    assert h.is_contiguous() and dout.is_contiguous()
+    D2 = h.shape[-1]
+    M = h.numel() // D2
+    assert dout.numel() == M * (D2 // 2)
+    dh = torch.empty_like(h)
+    check(lib().dm_geglu_bwd(bf, ptr_any(h), ptr_any(dout), M, D2 // 2, ptr_any(dh), stream_ptr()), "dm_geglu_bwd")
+    return dh
 
 
 def upsample2x(x, zero_insert=False):
@@ -514,3 +557,51 @@ def attention(q, k, v, heads, scale=None, out=None):
                              ptr_any(out), out.stride(1), out.stride(0), B, heads, Nq, Nk, 64, scale, stream_ptr()),
           "dm_attention")
     return out
+
+
+def _attn_views(q, k, v, heads):
+    B, Nq, Cq = q.shape
+    assert Cq == heads * 64 and k.shape[2] == Cq and v.shape[2] == Cq and k.shape[:2] == v.shape[:2] and k.shape[0] == B
+    assert q.stride(2) == 1 and k.stride(2) == 1 and v.stride(2) == 1
+    assert k.stride(1) == v.stride(1) and k.stride(0) == v.stride(0)
+    return B, Nq, k.shape[1], Cq
+
+
+def attention_lse(q, k, v, heads, scale=None, out=None):
+    """attention() that also returns lse [B, heads, Nq] fp32 = logsumexp_k(scale q.k) per query row, which attention_bwd
+    needs; the output is bit-identical to attention()'s.  16-bit storage only."""
+    bf = _is_bf16(q)    # fp32 storage: the library returns DM_EUNSUPPORTED
+    B, Nq, Nk, Cq = _attn_views(q, k, v, heads)
+    if out is None:
+        out = torch.empty(B, Nq, Cq, device=q.device, dtype=q.dtype)
+    lse = torch.empty(B, heads, Nq, device=q.device, dtype=torch.float32)
+    check(lib().dm_attention_lse(bf, ptr_any(q), q.stride(1), q.stride(0), ptr_any(k), ptr_any(v), k.stride(1), k.stride(0),
+                                 ptr_any(out), out.stride(1), out.stride(0), B, heads, Nq, Nk, 64,
+                                 1.0 / 8.0 if scale is None else scale, ptr_any(lse), stream_ptr()), "dm_attention_lse")
+    return out, lse
+
+
+def attention_bwd(q, k, v, o, do, lse, heads, scale=None, dq=None, dk=None, dv=None):
+    """Gradients (dq, dk, dv) of attention(q, k, v, heads, scale) = o for the output gradient do, from the lse of
+    attention_lse.  Every operand may be a token-major view with its own row / batch strides (last dim contiguous), as
+    attention() takes; dq / dk / dv given as column slices of one gradient buffer are written in place, its other columns
+    untouched.  16-bit storage only; deterministic."""
+    bf = _is_bf16(q)    # fp32 storage: the library returns DM_EUNSUPPORTED
+    B, Nq, Nk, Cq = _attn_views(q, k, v, heads)
+    assert o.shape == (B, Nq, Cq) and do.shape == (B, Nq, Cq) and lse.shape == (B, heads, Nq)
+    assert lse.dtype == torch.float32 and lse.is_contiguous()
+    if dq is None:
+        dq = torch.empty(B, Nq, Cq, device=q.device, dtype=q.dtype)
+    if dk is None:
+        dk = torch.empty(B, Nk, Cq, device=q.device, dtype=q.dtype)
+    if dv is None:
+        dv = torch.empty(B, Nk, Cq, device=q.device, dtype=q.dtype)
+    for t, shape in ((o, (B, Nq)), (do, (B, Nq)), (dq, (B, Nq)), (dk, (B, Nk)), (dv, (B, Nk))):
+        assert t.dtype == q.dtype and t.stride(2) == 1 and tuple(t.shape) == (*shape, Cq)
+    delta = torch.empty(B, heads, Nq, device=q.device, dtype=torch.float32)
+    check(lib().dm_attention_bwd(bf, ptr_any(q), q.stride(1), q.stride(0), ptr_any(k), ptr_any(v), k.stride(1), k.stride(0),
+                                 ptr_any(o), o.stride(1), o.stride(0), ptr_any(do), do.stride(1), do.stride(0), ptr_any(lse),
+                                 ptr_any(dq), dq.stride(1), dq.stride(0), ptr_any(dk), dk.stride(1), dk.stride(0),
+                                 ptr_any(dv), dv.stride(1), dv.stride(0), ptr_any(delta), B, heads, Nq, Nk, 64,
+                                 1.0 / 8.0 if scale is None else scale, stream_ptr()), "dm_attention_bwd")
+    return dq, dk, dv

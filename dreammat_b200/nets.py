@@ -148,27 +148,85 @@ class _UNetCommon(_Base):
             sc = x
         return D.conv2d(h, P[p + ".conv2.w"], 3, bias=P[p + ".conv2.bias"], residual=sc, out=out)
 
-    def transformer(self, p, x, ctx, heads):
+    def transformer(self, p, x, ctx, heads, tape=None):
+        """Transformer2DModel (one BasicTransformerBlock).  With a tape (a dict) it also records what transformer_bwd
+        needs; the output is the same bits either way (attention_lse writes attention's O)."""
         P, G = self.p, self.cfg.norm_groups
         n, H, W, C = x.shape
         M = n * H * W
-        hN, _ = D.groupnorm(x, P[p + ".norm.weight"], P[p + ".norm.bias"], G, 1e-6, silu=False)
-        h = D.gemm(hN.view(M, C), P[p + ".proj_in.w"], bias=P[p + ".proj_in.bias"])
+        attn = D.attention if tape is None else D.attention_lse
+        hN, stats = D.groupnorm(x, P[p + ".norm.weight"], P[p + ".norm.bias"], G, 1e-6, silu=False)
+        h0 = D.gemm(hN.view(M, C), P[p + ".proj_in.w"], bias=P[p + ".proj_in.bias"])
         b = p + ".transformer_blocks.0"
-        n1 = D.layernorm(h, P[b + ".norm1.weight"], P[b + ".norm1.bias"])
+        n1 = D.layernorm(h0, P[b + ".norm1.weight"], P[b + ".norm1.bias"])
         qkv = D.gemm(n1, P[b + ".attn1.qkv.w"]).view(n, H * W, 3 * C)
-        o = D.attention(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads)
-        h = D.gemm(o.view(M, C), P[b + ".attn1.to_out.0.w"], bias=P[b + ".attn1.to_out.0.bias"], residual=h)
-        n2 = D.layernorm(h, P[b + ".norm2.weight"], P[b + ".norm2.bias"])
+        o1 = attn(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads)
+        o1, lse1 = o1 if tape is not None else (o1, None)
+        h1 = D.gemm(o1.view(M, C), P[b + ".attn1.to_out.0.w"], bias=P[b + ".attn1.to_out.0.bias"], residual=h0)
+        n2 = D.layernorm(h1, P[b + ".norm2.weight"], P[b + ".norm2.bias"])
         q = D.gemm(n2, P[b + ".attn2.to_q.w"]).view(n, H * W, C)
         kv = D.gemm(ctx.view(-1, ctx.shape[-1]), P[b + ".attn2.kv.w"]).view(n, ctx.shape[1], 2 * C)
-        o = D.attention(q, kv[..., :C], kv[..., C:], heads)
-        h = D.gemm(o.view(M, C), P[b + ".attn2.to_out.0.w"], bias=P[b + ".attn2.to_out.0.bias"], residual=h)
-        n3 = D.layernorm(h, P[b + ".norm3.weight"], P[b + ".norm3.bias"])
+        o2 = attn(q, kv[..., :C], kv[..., C:], heads)
+        o2, lse2 = o2 if tape is not None else (o2, None)
+        h2 = D.gemm(o2.view(M, C), P[b + ".attn2.to_out.0.w"], bias=P[b + ".attn2.to_out.0.bias"], residual=h1)
+        n3 = D.layernorm(h2, P[b + ".norm3.weight"], P[b + ".norm3.bias"])
         f = D.gemm(n3, P[b + ".ff.net.0.proj.w"], bias=P[b + ".ff.net.0.proj.bias"], act="geglu")
-        h = D.gemm(f, P[b + ".ff.net.2.w"], bias=P[b + ".ff.net.2.bias"], residual=h)
+        h3 = D.gemm(f, P[b + ".ff.net.2.w"], bias=P[b + ".ff.net.2.bias"], residual=h2)
         xs = x if x.is_contiguous() else x.contiguous()
-        return D.gemm(h, P[p + ".proj_out.w"], bias=P[p + ".proj_out.bias"], residual=xs.view(M, C)).view(n, H, W, C)
+        if tape is not None:
+            tape.update(p=p, heads=heads, x=xs, ctx=ctx, hN=hN, stats=stats, h0=h0, n1=n1, qkv=qkv, o1=o1, lse1=lse1, h1=h1,
+                        n2=n2, q=q, kv=kv, o2=o2, lse2=lse2, h2=h2, n3=n3, f=f, h3=h3)
+        return D.gemm(h3, P[p + ".proj_out.w"], bias=P[p + ".proj_out.bias"], residual=xs.view(M, C)).view(n, H, W, C)
+
+    def transformer_bwd(self, rec, dout):
+        """Backward of transformer(p, x, ctx, heads, tape=rec) for the output gradient dout [n, H, W, C]: returns (dx,
+        grads), grads mapping each prepared parameter name of the block to its fp32 gradient in the prepared layout (qkv /
+        kv fused, ff.net.0.proj value / gate interleaved).  ctx gets no gradient (the text encoder is frozen).  The dgrad
+        GEMMs use W^T built here from the current weights, and the GEGLU pre-activation is recomputed by one GEMM."""
+        P, G, p, heads = self.p, self.cfg.norm_groups, rec["p"], rec["heads"]
+        b = p + ".transformer_blocks.0"
+        x = rec["x"]
+        n, H, W, C = x.shape
+        M = n * H * W
+        grads = {}
+
+        def lin(name, dy, xin, bias=True):
+            dw, db = D.gemm_wgrad(dy, xin, bias=bias)
+            grads[name + ".w"] = dw
+            if bias:
+                grads[name + ".bias"] = db
+            return D.gemm(dy.reshape(-1, dy.shape[-1]), D.transpose(P[name + ".w"]))
+
+        def ln(name, h, dn, dadd):
+            dh, grads[name + ".weight"], grads[name + ".bias"] = D.layernorm_bwd(h, dn, P[name + ".weight"], dx_add=dadd)
+            return dh
+
+        dy = dout.contiguous().view(M, C)
+        dh3 = lin(p + ".proj_out", dy, rec["h3"])
+        df = lin(b + ".ff.net.2", dh3, rec["f"])
+        g = D.gemm(rec["n3"], P[b + ".ff.net.0.proj.w"], bias=P[b + ".ff.net.0.proj.bias"])
+        dn3 = lin(b + ".ff.net.0.proj", D.geglu_bwd(g, df), rec["n3"])
+        dh2 = ln(b + ".norm3", rec["h2"], dn3, dh3)
+        do2 = lin(b + ".attn2.to_out.0", dh2, rec["o2"]).view(n, H * W, C)
+        kv = rec["kv"]
+        d_kv = torch.empty_like(kv)
+        dq2, _, _ = D.attention_bwd(rec["q"], kv[..., :C], kv[..., C:], rec["o2"], do2, rec["lse2"], heads,
+                                    dk=d_kv[..., :C], dv=d_kv[..., C:])
+        grads[b + ".attn2.kv.w"], _ = D.gemm_wgrad(d_kv, rec["ctx"])
+        dn2 = lin(b + ".attn2.to_q", dq2, rec["n2"], bias=False)
+        dh1 = ln(b + ".norm2", rec["h1"], dn2, dh2)
+        do1 = lin(b + ".attn1.to_out.0", dh1, rec["o1"]).view(n, H * W, C)
+        qkv = rec["qkv"]
+        d_qkv = torch.empty_like(qkv)
+        D.attention_bwd(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], rec["o1"], do1, rec["lse1"], heads,
+                        dq=d_qkv[..., :C], dk=d_qkv[..., C:2 * C], dv=d_qkv[..., 2 * C:])
+        dn1 = lin(b + ".attn1.qkv", d_qkv, rec["n1"], bias=False)
+        dh0 = ln(b + ".norm1", rec["h0"], dn1, dh1)
+        dhN = lin(p + ".proj_in", dh0, rec["hN"].view(M, C)).view(n, H, W, C)
+        gm, bt = P[p + ".norm.weight"], P[p + ".norm.bias"]
+        dx = D.groupnorm_bwd(x, dhN, gm, bt, rec["stats"], G, 1e-6, dx_add=dout.contiguous())
+        grads[p + ".norm.weight"], grads[p + ".norm.bias"] = D.groupnorm_affine_grad(x, dhN, gm, bt, rec["stats"], G)
+        return dx, grads
 
     def down_and_mid(self, sample, tproj, ctx):
         cfg = self.cfg

@@ -17,9 +17,11 @@
  * a summation order).  Still accumulated with fp32 atomics: the logged sums (norms of dm_conv2d_csd / dm_sds_grad, reg_sums
  * of the shading) and the adjoint of dm_resize_bilinear (renders that are not 512^2).  Weight gradients (dm_conv2d_wgrad /
  * dm_gemm_wgrad) sum each element in one fixed K order, split-K slices in slice order, and the bias gradient's per-block
- * partial rows in row order.  dm_groupnorm / dm_groupnorm_bwd (per-block partial sums), the bias gradient of
+ * partial rows in row order.  dm_attention_bwd gives every dQ / dK / dV element to one CTA, which sums its blocks in
+ * order (S and dP are recomputed rather than dQ added atomically); its delta scratch comes from the caller.  dm_groupnorm / dm_groupnorm_bwd (per-block partial sums), the bias gradient of
  * dm_conv2d_wgrad / dm_gemm_wgrad (per-block partial rows), dm_antialias_fwd / _bwd (per-pixel pair buckets) and
- * dm_hashgrid_mlp_bwd (int64 fixed-point grid gradient) need scratch for that which their signatures have no room for; the library allocates it once per device, on
+ * dm_hashgrid_mlp_bwd (int64 fixed-point grid gradient), dm_layernorm_bwd / dm_groupnorm_affine_grad (per-chunk partial
+ * rows of the affine gradients) need scratch for that which their signatures have no room for; the library allocates it once per device, on
  * the first call (not while the stream is being captured: run a call once before capturing it), and never frees it.  Calls
  * on one device must not run concurrently on two streams.
  */
@@ -301,8 +303,24 @@ int dm_groupnorm_bwd(int bf16, const void* x, const void* dz, int n_img, int HW,
                      void* dx, void* stream);
 int dm_layernorm(int bf16, const void* x, int64_t M, int C, const void* gamma, const void* beta, float eps, void* y,
                  void* stream);
+/* LayerNorm backward (eps as the forward): dx = d/dx LN(x) . dy (+ dx_add) in the storage dtype; dgamma, dbeta [C] fp32
+ * (overwritten).  Mean and rstd are recomputed from x.  x, dy, dx_add, dx dense [M, C], C % 8 == 0, C <= 1280.  The
+ * affine gradients add per-chunk partial rows (library scratch, see DETERMINISM) in chunk order.  16-bit only: bf16 == 2
+ * returns DM_EUNSUPPORTED. */
+int dm_layernorm_bwd(int bf16, const void* x, const void* dy, int64_t M, int C, const void* gamma, float eps,
+                     const void* dx_add, void* dx, float* dgamma, float* dbeta, void* stream);
+/* GroupNorm affine gradients: dgamma[c] = sum dz' xhat, dbeta[c] = sum dz' over every pixel of every image, dz' = dz, or
+ * dz * silu'(y) with silu = 1 (GroupNorm + SiLU); x, dz dense [n_img, HW, C]; stats as dm_groupnorm returns them.  dx comes
+ * from dm_groupnorm_bwd.  Deterministic as dm_layernorm_bwd; 16-bit only (bf16 == 2: DM_EUNSUPPORTED). */
+int dm_groupnorm_affine_grad(int bf16, const void* x, const void* dz, int n_img, int HW, int C, int G, const void* gamma,
+                             const void* beta, int silu, const float* stats, float* dgamma, float* dbeta, void* stream);
 /* out[m,j] = h[m,j] * gelu(h[m,D+j]), h [M,2D] */
 int dm_geglu(int bf16, const void* h, int64_t M, int D, void* out, void* stream);
+/* GEGLU backward on the interleaved pre-activation the fused GEGLU epilogue of dm_gemm consumes (h [M, 2D] in 64-column
+ * blocks: 32 value columns, then their 32 gate columns; out[m, 32b+r] = h[m, 64b+r] * gelu(h[m, 64b+32+r]), erf GELU):
+ * dh [M, 2D] in the same layout, so dh feeds dm_gemm_wgrad / the dgrad GEMM against the interleaved weight.  D % 32 == 0;
+ * 16-bit only (bf16 == 2: DM_EUNSUPPORTED). */
+int dm_geglu_bwd(int bf16, const void* h, const void* dout, int64_t M, int D, void* dh, void* stream);
 /* nearest 2x (zero_insert=0) or zero-insertion 2x (zero_insert=1, adjoint of a stride-2 gather) */
 int dm_upsample2x(int bf16, const void* x, int n, int H, int W, int C, int zero_insert, void* y, void* stream);
 /* dst[r,0:cols] = a*s1[r,0:cols] + b*s2[r,0:cols] (s2 may be NULL) with independent row strides */
@@ -340,6 +358,27 @@ int dm_silu(int bf16, const void* x, int64_t n, void* y, void* stream);
 int dm_attention(int bf16, const void* q, int64_t ldq, int64_t q_batch_stride, const void* k, const void* v,
                  int64_t ldkv, int64_t kv_batch_stride, void* out, int64_t ldo, int64_t out_batch_stride, int batch,
                  int heads, int Nq, int Nk, int head_dim, float scale, void* stream);
+/* dm_attention that also writes lse [batch, heads, Nq] fp32 = logsumexp_k(scale * q.k) (natural log) per query row: what
+ * dm_attention_bwd needs to recompute P.  O is bit-identical to dm_attention's.  16-bit storage only: bf16 == 2 returns
+ * DM_EUNSUPPORTED. */
+int dm_attention_lse(int bf16, const void* q, int64_t ldq, int64_t q_batch_stride, const void* k, const void* v,
+                     int64_t ldkv, int64_t kv_batch_stride, void* out, int64_t ldo, int64_t out_batch_stride, int batch,
+                     int heads, int Nq, int Nk, int head_dim, float scale, float* lse, void* stream);
+/* Backward of dm_attention (the q / k / v gradients autograd computes through SDPA): dQ, dK, dV (storage dtype,
+ * overwritten) from q, k, v, the forward's O, dO and the lse of dm_attention_lse.  Every operand has its own row stride
+ * and batch stride, head h in columns [64h, 64h+64), so dQ / dK / dV can be column slices of one fused [B, N, 3C] or
+ * [B, Nk, 2C] gradient buffer (other columns are left untouched).  delta is caller scratch of batch*heads*Nq floats
+ * (rowsum(dO o O)).  Three kernels, no atomics: delta, then one CTA per 128 keys (dK, dV) and one per 128 queries (dQ);
+ * S and dP are computed in both, which is the price of every output element having one owner.  P and dS are rounded
+ * to the storage type before their products, accumulation is fp32.  head_dim 64, fp16 / bf16 only (bf16 == 2 returns
+ * DM_EUNSUPPORTED); strides must be multiples of 8 elements (row strides >= heads*64), the 16-bit operands 16-byte
+ * aligned, lse / delta 4-byte aligned, else DM_EINVAL before any launch.  Deterministic. */
+int dm_attention_bwd(int bf16, const void* q, int64_t ldq, int64_t q_batch_stride, const void* k, const void* v,
+                     int64_t ldkv, int64_t kv_batch_stride, const void* o, int64_t ldo, int64_t o_batch_stride,
+                     const void* dout, int64_t lddo, int64_t do_batch_stride, const float* lse, void* dq, int64_t lddq,
+                     int64_t dq_batch_stride, void* dk, int64_t lddk, int64_t dk_batch_stride, void* dv, int64_t lddv,
+                     int64_t dv_batch_stride, float* delta, int batch, int heads, int Nq, int Nk, int head_dim,
+                     float scale, void* stream);
 
 #ifdef __cplusplus
 }
