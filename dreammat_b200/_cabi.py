@@ -108,6 +108,10 @@ SIGNATURES = {
     "dm_conv2d": (C.c_int, [C.c_int, P] + [C.c_int] * 4 + [P] + [C.c_int] * 7 + [P, I64, P, C.c_int, P]),
     "dm_conv2d_wgrad": (C.c_int, [C.c_int, P] + [C.c_int] * 4 + [P, I64] + [C.c_int] * 7 + [P, P, P]),
     "dm_gemm_wgrad": (C.c_int, [C.c_int, P, I64, P, I64, C.c_int, C.c_int, C.c_int, P, P, P]),
+    "dm_conv2d_dgrad": (C.c_int, [C.c_int, P] + [C.c_int] * 4 + [P] + [C.c_int] * 4 + [P, I64, P, C.c_int, P]),
+    "dm_gemm_dgrad": (C.c_int, [C.c_int, P, I64, P, I64, P, I64, C.c_int, C.c_int, C.c_int, P, C.c_int, P]),
+    "dm_silu_bwd": (C.c_int, [C.c_int, P, P, I64, P, P]),
+    "dm_rowvec_grad": (C.c_int, [C.c_int, P, I64, C.c_int, C.c_int, C.c_int, P, I64, P]),
 }
 
 

@@ -15,7 +15,7 @@ void dm_set_error(const char* fmt, ...);
 void dm_count_launch();
 
 // Library-owned device scratch of the deterministic reductions (GroupNorm partial rows, the hash-grid backward's fixed-point
-// accumulator, the bias-gradient partial rows of the weight gradients, the norm affine-gradient partial rows): one buffer per device and slot, zero-filled when
+// accumulator, the bias-gradient partial rows of the weight gradients, the norm affine-gradient and rowvec-gradient partial rows): one buffer per device and slot, zero-filled when
 // allocated.  Callers of one device must not use a slot from two streams at once (the same rule as the split-K workspace).
 // A buffer is never freed, because a captured CUDA graph may hold its address; it can only grow outside stream capture (a
 // warm-up call before capture sizes it).  Returns nullptr with the error set on failure.

@@ -708,6 +708,60 @@ __global__ void __launch_bounds__(256) silu_kernel(const T* __restrict__ x, int6
         y[i] = H<T>::t(silu_f(H<T>::f(x[i])));
 }
 
+// dx = dy * silu'(z) on the pre-activation z (the backward of a SiLU epilogue whose pre-activation was recomputed)
+template <typename T>
+__global__ void __launch_bounds__(256) silu_bwd_kernel(const T* __restrict__ z, const T* __restrict__ dy, int64_t n8,
+                                                       T* __restrict__ dx) {
+    griddep_launch_dependents();
+    griddep_wait();
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint4 uz = reinterpret_cast<const uint4*>(z)[i], ud = reinterpret_cast<const uint4*>(dy)[i];
+        const T* hz = reinterpret_cast<const T*>(&uz); const T* hd = reinterpret_cast<const T*>(&ud);
+        uint4 o; T* oh = reinterpret_cast<T*>(&o);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) oh[j] = H<T>::t(H<T>::f(hd[j]) * silu_grad(H<T>::f(hz[j])));
+        reinterpret_cast<uint4*>(dx)[i] = o;
+    }
+}
+
+// Gradient of the GEMM epilogue's per-image vector (a resnet's slice of the time-embedding projection): out[img, c] = sum
+// over the image's rows of dy[row, c].  Block (v-block, chunk, img): a thread owns one 8-channel vector and the chunk's
+// rows [chunk*rpc, +rpc) and writes its sums to partial row part[img][chunk][N]; rowvec_finish_kernel adds an image's
+// partial rows in chunk order, so the result is bit-identical from run to run.
+template <typename T>
+__global__ void __launch_bounds__(128) rowvec_partials_kernel(const T* __restrict__ dy, int64_t ld, int rows_per_img, int N,
+                                                              int rpc, float* __restrict__ part) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= N / 8) return;
+    const int r0 = blockIdx.y * rpc, r1 = min(rows_per_img, r0 + rpc);
+    const T* base = dy + (int64_t)blockIdx.z * rows_per_img * ld + 8 * v;
+    float s[8] = {};
+    for (int r = r0; r < r1; ++r) {
+        const uint4 u = *reinterpret_cast<const uint4*>(base + r * ld);
+        const T* h = reinterpret_cast<const T*>(&u);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s[k] += H<T>::f(h[k]);
+    }
+    float* pr = part + ((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * N + 8 * v;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) pr[k] = s[k];
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) rowvec_finish_kernel(const float* __restrict__ part, int chunks, int N, int n_img,
+                                                            T* __restrict__ out, int64_t ld_out) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n_img * N) return;
+    const int img = j / N, c = j - img * N;
+    float s = 0.f;
+    for (int k = 0; k < chunks; ++k) s += part[((int64_t)img * chunks + k) * N + c];
+    out[img * ld_out + c] = H<T>::t(s);
+}
+
 // ----------------------------------------------------------------------------------- norm / GEGLU backward
 // LayerNorm backward, warp per row (the forward's mapping): mean / rstd recomputed from x with the forward's arithmetic,
 // g = dy * gamma, dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dx_add).  (mean, rstd) of each row go to `rstats`
@@ -1099,6 +1153,43 @@ extern "C" int dm_silu(int bf16, const void* x, int64_t n, void* y, void* stream
     DM_DTYPE_OK(bf16);
     DM_REQUIRE(x && y, "null pointer");
     DM_DISPATCH_T3(bf16, silu_kernel<T><<<grid_for(n), 256, 0, (cudaStream_t)stream>>>((const T*)x, n, (T*)y));
+    DM_CHECK_LAUNCH();
+    return DM_OK;
+}
+
+extern "C" int dm_silu_bwd(int bf16, const void* z, const void* dy, int64_t n, void* dx, void* stream) {
+    DM_DTYPE_OK(bf16);
+    if (bf16 == 2) { dm_set_error("dm_silu_bwd: fp32 storage is not supported (16-bit only)"); return DM_EUNSUPPORTED; }
+    DM_REQUIRE(z && dy && dx, "null pointer");
+    DM_REQUIRE(n >= 0 && n % 8 == 0 && ((((uintptr_t)z | (uintptr_t)dy | (uintptr_t)dx) & 15) == 0),
+               "element count a multiple of 8, 16-byte aligned operands");
+    if (n == 0) return DM_OK;
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(silu_bwd_kernel<T>, dim3((unsigned)grid_for(n / 8)), dim3(256), 0, (cudaStream_t)stream,
+                                                (const T*)z, (const T*)dy, n / 8, (T*)dx)));
+    DM_CHECK_LAUNCH();
+    return DM_OK;
+}
+
+extern "C" int dm_rowvec_grad(int bf16, const void* dy, int64_t ld, int n_img, int rows_per_img, int N, void* out,
+                              int64_t ld_out, void* stream) {
+    DM_DTYPE_OK(bf16);
+    if (bf16 == 2) { dm_set_error("dm_rowvec_grad: fp32 storage is not supported (16-bit only)"); return DM_EUNSUPPORTED; }
+    DM_REQUIRE(dy && out, "null pointer");
+    DM_REQUIRE(n_img > 0 && rows_per_img > 0 && N > 0 && N % 8 == 0, "positive extents, N a multiple of 8");
+    DM_REQUIRE(ld % 8 == 0 && ld >= N && ((uintptr_t)dy & 15) == 0, "dy 16-byte aligned, row stride a multiple of 8 elements, at least N");
+    DM_REQUIRE(ld_out >= N && ((uintptr_t)out & 1) == 0, "out row stride at least N");
+    cudaStream_t st = (cudaStream_t)stream;
+    // about 4 CTAs per SM over (images x chunks), at least 16 rows per chunk
+    int rpc = (int)dm_ceil_div((int64_t)n_img * rows_per_img, DM_NUM_SMS * 4);
+    if (rpc < 16) rpc = 16;
+    const int chunks = (int)dm_ceil_div(rows_per_img, rpc);
+    float* part = (float*)dm_scratch(DM_SCRATCH_AFFINE, (size_t)n_img * chunks * N * sizeof(float), st);
+    if (!part) return DM_EDRIVER;
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(rowvec_partials_kernel<T>, dim3((unsigned)dm_ceil_div(N / 8, 128), (unsigned)chunks, (unsigned)n_img),
+                                                dim3(128), 0, st, (const T*)dy, ld, rows_per_img, N, rpc, part)));
+    DM_CHECK_LAUNCH();
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(rowvec_finish_kernel<T>, dim3((unsigned)dm_ceil_div((int64_t)n_img * N, 256)), dim3(256), 0, st,
+                                                (const float*)part, chunks, N, n_img, (T*)out, ld_out)));
     DM_CHECK_LAUNCH();
     return DM_OK;
 }

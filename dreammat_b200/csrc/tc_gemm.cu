@@ -25,8 +25,10 @@
 // residual boxes are loaded into a shared output tile, combined in place and stored as boxes (see the epilogue role).
 // choose_tile() picks the tile width and split-K.
 //
-// Weight gradients (dm_conv2d_wgrad / dm_gemm_wgrad) run the same kernel in its WG mode: D[Cout, taps*Cin] (fp32) reduces
+// Weight gradients (dm_conv2d_wgrad / dm_gemm_wgrad) run the same kernel in its WGRAD mode: D[Cout, taps*Cin] (fp32) reduces
 // over the pixel / token axis, with both operands MN-major boxes of the NHWC / token-major dY and x (see WG_BOX).
+// Input gradients (dm_conv2d_dgrad / dm_gemm_dgrad) run it in its DGRAD mode: A = dY exactly as a forward activation, B =
+// MN-major boxes of the forward weight itself (see MODE_DGRAD), so no flipped / transposed weight copy ever exists.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -347,14 +349,25 @@ template <int BN> struct Cfg {
 constexpr int WG_BOX = 64 * 128;                     // bytes of one 64-channel x 64-pixel box
 constexpr int WG_PIX = 64;                           // pixels per K-block
 
+// Input-gradient mode (DGRAD): D[M = pixels (tokens), N = Cin (K_in)] = sum over K = (tap, co) of dY . W, with the B
+// operand read from the forward weight W[Cout, taps*Cin] ([N_out, K_in] for a linear) as it is.  A is dY, K-major, loaded
+// like a forward activation (a conv shifts it by k-1-pad, the host passes that as the padding).  For K-block (tap, 64
+// output channels co) and the tile's input channels ci0.., B is BN / 64 MN-major boxes of 64 contiguous ci x 64 rows co
+// at column (taps-1-tap)*Cin + ci0: the tap flip of the transposed convolution is a coordinate.  The K order (tap-major,
+// then co) and every product are those of the forward kernel on a flipped, transposed weight copy, so the result is
+// bit-identical to it.  Columns of a box past Cin hold the next tap's weights (or TMA zeros): they only reach output
+// columns >= N, which the epilogue drops.
+constexpr int MODE_FWD = 0, MODE_WGRAD = 1, MODE_DGRAD = 2;
+
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...
-template <int BN, typename T, bool WG = false>
+template <int BN, typename T, int MODE = MODE_FWD>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
                                                              const __grid_constant__ CUtensorMap tmB,
                                                              const __grid_constant__ CUtensorMap tmO,
                                                              const __grid_constant__ CUtensorMap tmR,
                                                              const GemmParams p) {
     using C = Cfg<BN>;
+    constexpr bool WG = MODE == MODE_WGRAD, DG = MODE == MODE_DGRAD;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;
@@ -452,15 +465,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
                     mbar_wait(empty_bar(stage), phase ^ 1u);
                     const uint32_t a_dst = smem_base + stage * C::STAGE_BYTES;
                     const uint32_t b_dst = a_dst + C::A_BYTES;
-                    mbar_expect_tx(full_bar(stage), C::STAGE_BYTES);
+                    // DGRAD: weight boxes wholly past N are not loaded (they would only feed columns the epilogue drops)
+                    const int b_boxes = DG ? min(BN / 64, (p.N - n_tile * BN + 63) / 64) : 0;
+                    mbar_expect_tx(full_bar(stage), DG ? (uint32_t)(C::A_BYTES + b_boxes * WG_BOX) : (uint32_t)C::STAGE_BYTES);
+                    int tap = 0, slab = kb;
                     if (p.is_conv) {
-                        int tap = kb / slabs, slab = kb - tap * slabs;
+                        tap = kb / slabs; slab = kb - tap * slabs;
                         int kh = tap / p.kw_n, kw = tap - kh * p.kw_n;
                         tma_load_4d(a_dst, &tmA, full_bar(stage), slab * BK, c_w + kw, c_h + kh, c_n);
                     } else {
                         tma_load_3d(a_dst, &tmA, full_bar(stage), kb * BK, m_tile * BM, z);
                     }
-                    tma_load_3d(b_dst, &tmB, full_bar(stage), kb * BK, n_tile * BN, p.b_batched ? z : 0);
+                    if constexpr (DG) {
+                        for (int j = 0; j < b_boxes; ++j)
+                            tma_load_3d(b_dst + j * WG_BOX, &tmB, full_bar(stage), (p.taps - 1 - tap) * p.N + n_tile * BN + 64 * j, slab * BK, 0);
+                    } else {
+                        tma_load_3d(b_dst, &tmB, full_bar(stage), kb * BK, n_tile * BN, p.b_batched ? z : 0);
+                    }
                     if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
                 }
             }
@@ -548,12 +569,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_gemm_kernel(const __grid_const
             // pixel rows is +2048 bytes (+128 in the descriptor's 16-byte units)
             const uint64_t da = WG ? make_sw128_desc_mn(a_addr + (uint32_t)wg * WG_BOX, WG_BOX)
                                    : make_sw128_desc(a_addr + (uint32_t)wg * (64 * 128));
-            const uint64_t db = WG ? make_sw128_desc_mn(a_addr + C::A_BYTES, WG_BOX) : make_sw128_desc(a_addr + C::A_BYTES);
+            const uint64_t db = (WG || DG) ? make_sw128_desc_mn(a_addr + C::A_BYTES, WG_BOX) : make_sw128_desc(a_addr + C::A_BYTES);
             wgmma_fence();
             wgmma_fence_operands(acc);
 #pragma unroll
             for (int k = 0; k < BK / 16; ++k) {
                 if constexpr (WG) Wgmma<BN, T>::ss_tt(acc, da + (uint64_t)(128 * k), db + (uint64_t)(128 * k));
+                else if constexpr (DG) Wgmma<BN, T>::ss_nt(acc, da + (uint64_t)(2 * k), db + (uint64_t)(128 * k));
                 else Wgmma<BN, T>::ss(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k));
             }
             wgmma_commit();
@@ -630,11 +652,11 @@ int out_map(CUtensorMap* m, int bf16, const void* base, int n, int M, int batch,
     return encode_map(m, bf16, base, 3, dims, str, box, es, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
-template <int BN, typename T, bool WG = false>
+template <int BN, typename T, int MODE = MODE_FWD>
 int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR,
            const GemmParams& p, int64_t work_items, cudaStream_t st) {
     static bool configured = false;
-    auto kern = tc_gemm_kernel<BN, T, WG>;
+    auto kern = tc_gemm_kernel<BN, T, MODE>;
     if (!configured) {
         DM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM));
         configured = true;
@@ -781,7 +803,7 @@ int pick_split(int64_t tiles, int nk, int64_t mn, int N, int act) {
 TileChoice choose_tile(int64_t M, int N, int bn_hint) { return {pick_bn(M, N, bn_hint), 0}; }
 
 int dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p_in, const TileChoice& tc, int bf16, cudaStream_t st,
-             bool wgrad = false) {
+             int mode = MODE_FWD) {
     GemmParams p = p_in;
     const int64_t batch = p.batch > 0 ? p.batch : 1;
     const int64_t tiles = dm_ceil_div(p.N, tc.bn) * dm_ceil_div(p.M, BM) * batch;
@@ -804,9 +826,12 @@ int dispatch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p
         }
     }
     const int64_t work = tiles * split;
-    if (wgrad) {
-        if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16, true>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half, true>(tmA, tmB, tmO, tmR, p, work, st);
-        else rc = bf16 ? launch<128, __nv_bfloat16, true>(tmA, tmB, tmO, tmR, p, work, st) : launch<128, __half, true>(tmA, tmB, tmO, tmR, p, work, st);
+    if (mode == MODE_WGRAD) {
+        if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16, MODE_WGRAD>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half, MODE_WGRAD>(tmA, tmB, tmO, tmR, p, work, st);
+        else rc = bf16 ? launch<128, __nv_bfloat16, MODE_WGRAD>(tmA, tmB, tmO, tmR, p, work, st) : launch<128, __half, MODE_WGRAD>(tmA, tmB, tmO, tmR, p, work, st);
+    } else if (mode == MODE_DGRAD) {
+        if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16, MODE_DGRAD>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half, MODE_DGRAD>(tmA, tmB, tmO, tmR, p, work, st);
+        else rc = bf16 ? launch<128, __nv_bfloat16, MODE_DGRAD>(tmA, tmB, tmO, tmR, p, work, st) : launch<128, __half, MODE_DGRAD>(tmA, tmB, tmO, tmR, p, work, st);
     } else if (tc.bn == 64) rc = bf16 ? launch<64, __nv_bfloat16>(tmA, tmB, tmO, tmR, p, work, st) : launch<64, __half>(tmA, tmB, tmO, tmR, p, work, st);
     else rc = bf16 ? launch<128, __nv_bfloat16>(tmA, tmB, tmO, tmR, p, work, st) : launch<128, __half>(tmA, tmB, tmO, tmR, p, work, st);
     if (rc || split <= 1) return rc;
@@ -840,7 +865,7 @@ int wgrad_run(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, int
     p.batch = 1;
     p.out = dw; p.ldc = p.N; p.out_f32 = 1;
     p.alpha = 1.0f; p.out_scale = 1.0f; p.rows_per_vec = 1;
-    return dispatch(tmA, tmB, p, choose_tile(p.M, p.N, 0), bf16, st, true);
+    return dispatch(tmA, tmB, p, choose_tile(p.M, p.N, 0), bf16, st, MODE_WGRAD);
 }
 
 }  // namespace
@@ -1038,6 +1063,93 @@ extern "C" int dm_gemm_wgrad(int bf16, const void* dy, int64_t ld_dy, const void
     int rc = wgrad_run(tmA, tmB, p, bf16, dw, st);
     if (rc || !db) return rc;
     return bias_grad(bf16, dy, ld_dy, M, N, db, st);
+}
+
+// ---- input gradients.  Both plan like the forward contraction they equal (dm_gemm_plan(M, N = Cin / K_in, K = taps*Cout /
+// N_out, act, bn_hint) reports the tile and split), and honour the whole dm_epilogue.
+static int dgrad_storage_check(int bf16, const char* name) {
+    if (bf16 == 2) {
+        dm_set_error("%s: input gradients in fp32 storage (high-precision mode) are not implemented", name);
+        return DM_EUNSUPPORTED;
+    }
+    DM_REQUIRE(bf16 == 0 || bf16 == 1, "storage selector: 0 fp16, 1 bf16");
+    return DM_OK;
+}
+// B operand of the DGRAD mode: the forward weight [rows, ld] (first `cols` columns) as boxes of 64 columns x 64 rows
+static int dgrad_weight_map(CUtensorMap* m, int bf16, const void* w, int64_t cols, int64_t rows, int64_t ld) {
+    uint64_t dims[3] = {(uint64_t)cols, (uint64_t)rows, 1};
+    uint64_t str[2] = {(uint64_t)ld * 2, (uint64_t)rows * ld * 2};
+    uint32_t box[3] = {64, BK, 1}, es[3] = {1, 1, 1};
+    return encode_map(m, bf16, w, 3, dims, str, box, es);
+}
+static int dgrad_epilogue_check(const dm_epilogue* ep, const void* dx, int64_t ldc, int N) {
+    const int per16 = (ep && ep->out_f32) ? 4 : 8;      // elements per 16 bytes of dx
+    DM_REQUIRE(((uintptr_t)dx & 15) == 0 && ldc >= N && ldc % per16 == 0,
+               "dx 16-byte aligned, row stride at least the gradient's width and a multiple of 16 bytes");
+    DM_REQUIRE(!ep || ep->act != 3, "the GEGLU epilogue has no meaning for an input gradient");
+    DM_REQUIRE(!ep || !ep->residual || ep->ld_res == 0 || ep->ld_res >= N, "residual row stride at least the gradient's width");
+    return DM_OK;
+}
+
+extern "C" int dm_conv2d_dgrad(int bf16, const void* dy, int n_img, int H, int W, int Cout, const void* w, int Cin, int ksize,
+                               int pad_t, int pad_l, void* dx, int64_t ldc, const dm_epilogue* ep, int bn_hint, void* stream) {
+    if (int rc = dgrad_storage_check(bf16, "dm_conv2d_dgrad")) return rc;
+    DM_REQUIRE(dy && w && dx, "null pointer");
+    DM_REQUIRE((((uintptr_t)dy | (uintptr_t)w) & 15) == 0, "dy and w 16-byte aligned");
+    DM_REQUIRE(n_img > 0 && H > 0 && W > 0, "positive extents");
+    DM_REQUIRE(Cout > 0 && Cout % BK == 0, "Cout must be a multiple of 64 (it is the reduction axis)");
+    DM_REQUIRE(Cin > 0 && Cin % 8 == 0, "Cin must be a multiple of 8");
+    DM_REQUIRE(ksize == 3 || ksize == 1, "3x3 or 1x1");
+    DM_REQUIRE(pad_t >= 0 && pad_t < ksize && pad_l >= 0 && pad_l < ksize, "padding of the forward convolution: 0 .. ksize-1");
+    if (int rc = dgrad_epilogue_check(ep, dx, ldc, Cin)) return rc;
+    int tile_w = W < BM ? W : BM;
+    int tile_h = (BM / tile_w) < H ? (BM / tile_w) : H;
+    int tile_n = BM / (tile_w * tile_h);
+    DM_REQUIRE(tile_w * tile_h * tile_n == BM && W % tile_w == 0 && H % tile_h == 0,
+               "extent must tile into 128-pixel boxes (power-of-two sizes)");
+    const int taps = ksize * ksize;
+    TileChoice tc = choose_tile((int64_t)n_img * H * W, Cin, bn_hint);
+    CUtensorMap tmA, tmB;
+    {
+        uint64_t dims[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)n_img};
+        uint64_t str[3] = {(uint64_t)Cout * 2, (uint64_t)W * Cout * 2, (uint64_t)H * W * Cout * 2};
+        uint32_t box[4] = {BK, (uint32_t)tile_w, (uint32_t)tile_h, (uint32_t)tile_n}, es[4] = {1, 1, 1, 1};
+        int rc = encode_map(&tmA, bf16, dy, 4, dims, str, box, es); if (rc) return rc;
+    }
+    if (int rc = dgrad_weight_map(&tmB, bf16, w, (int64_t)taps * Cin, Cout, (int64_t)taps * Cin)) return rc;
+    GemmParams p; memset(&p, 0, sizeof(p));
+    p.M = n_img * H * W; p.N = Cin; p.K = taps * Cout; p.batch = 1; p.is_conv = 1; p.Cin = Cout; p.taps = taps; p.kw_n = ksize;
+    p.Ho = H; p.Wo = W; p.tile_w = tile_w; p.tile_h = tile_h; p.tile_n = tile_n; p.stride = 1;
+    p.pad_t = ksize - 1 - pad_t; p.pad_l = ksize - 1 - pad_l;
+    p.out = dx; p.ldc = (int)ldc; p.out_batch_stride = 0;
+    fill_epilogue(p, ep, Cin);
+    return dispatch(tmA, tmB, p, tc, bf16, (cudaStream_t)stream, MODE_DGRAD);
+}
+
+extern "C" int dm_gemm_dgrad(int bf16, const void* dy, int64_t ld_dy, const void* w, int64_t ldw, void* dx, int64_t ldc, int M,
+                             int N_out, int K_in, const dm_epilogue* ep, int bn_hint, void* stream) {
+    if (int rc = dgrad_storage_check(bf16, "dm_gemm_dgrad")) return rc;
+    DM_REQUIRE(dy && w && dx, "null pointer");
+    DM_REQUIRE((((uintptr_t)dy | (uintptr_t)w) & 15) == 0, "dy and w 16-byte aligned");
+    DM_REQUIRE(M > 0 && N_out > 0 && N_out % BK == 0 && K_in > 0 && K_in % 8 == 0,
+               "M >= 1, N_out a positive multiple of 64 (it is the reduction axis), K_in a multiple of 8");
+    DM_REQUIRE(ld_dy % 8 == 0 && ldw % 8 == 0 && ld_dy >= N_out && ldw >= K_in,
+               "row strides: multiples of 8 elements (16 bytes), at least N_out (dy) and K_in (w)");
+    if (int rc = dgrad_epilogue_check(ep, dx, ldc, K_in)) return rc;
+    TileChoice tc = choose_tile(M, K_in, bn_hint);
+    CUtensorMap tmA, tmB;
+    {
+        uint64_t dims[3] = {(uint64_t)N_out, (uint64_t)M, 1};
+        uint64_t str[2] = {(uint64_t)ld_dy * 2, (uint64_t)M * ld_dy * 2};
+        uint32_t box[3] = {BK, BM, 1}, es[3] = {1, 1, 1};
+        int rc = encode_map(&tmA, bf16, dy, 3, dims, str, box, es); if (rc) return rc;
+    }
+    if (int rc = dgrad_weight_map(&tmB, bf16, w, K_in, N_out, ldw)) return rc;
+    GemmParams p; memset(&p, 0, sizeof(p));
+    p.M = M; p.N = K_in; p.K = N_out; p.batch = 1; p.taps = 1;
+    p.out = dx; p.ldc = (int)ldc; p.out_batch_stride = 0;
+    fill_epilogue(p, ep, K_in);
+    return dispatch(tmA, tmB, p, tc, bf16, (cudaStream_t)stream, MODE_DGRAD);
 }
 
 

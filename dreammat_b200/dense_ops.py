@@ -253,6 +253,57 @@ def gemm_wgrad(dy, x, bias=False):
     return dw, db
 
 
+def conv2d_dgrad(dy, w, ksize, pad=(1, 1), cin=None, residual=None, alpha=1.0, out_scale=1.0, out=None, out_f32=False, bn=0):
+    """Input gradient of the stride-1 conv2d(x, w, ksize, pad=pad) for the output gradient dy [n,H,W,Cout] (contiguous),
+    read from the forward weight w [Cout, k*k*Cin] itself: dx [n,H,W,Cin] (+ residual, a second gradient branch), or into
+    `out`, which may be a channel slice of a wider buffer.  cin defaults to w's.  A stride-2 forward is differentiated by
+    upsample2x(dy, zero_insert=True) followed by this.  16-bit storage only."""
+    _ensure_workspace()
+    bf = _wgrad_storage(dy)
+    assert w.dtype == dy.dtype and dy.is_contiguous() and w.is_contiguous()
+    n, H, W, Cout = dy.shape
+    taps = ksize * ksize
+    assert w.shape[0] == Cout and w.shape[1] % taps == 0
+    Cin = w.shape[1] // taps
+    assert cin is None or cin == Cin, "cin must be the channel count of the weight's layout"
+    if out is None:
+        out = torch.empty(n, H, W, Cin, device=dy.device, dtype=torch.float32 if out_f32 else dy.dtype)
+    assert out.stride(-1) == 1 and tuple(out.shape) == (n, H, W, Cin)
+    ldc = out.stride(2)
+    assert out.stride(1) == W * ldc and out.stride(0) == H * W * ldc
+    ld_res = 0
+    if residual is not None:
+        ld_res = residual.stride(2)
+        assert residual.stride(-1) == 1 and residual.stride(1) == W * ld_res and residual.stride(0) == H * W * ld_res
+    e = _ep(None, None, H * W, residual, ld_res, 0, alpha, out_scale, None, out.dtype == torch.float32)
+    check(lib().dm_conv2d_dgrad(bf, ptr_any(dy), n, H, W, Cout, ptr_any(w), Cin, ksize, pad[0], pad[1], ptr_any(out), ldc,
+                                C.byref(e), bn, stream_ptr()), "dm_conv2d_dgrad")
+    return out
+
+
+def gemm_dgrad(dy, w, residual=None, alpha=1.0, out_scale=1.0, out=None, out_f32=False, bn=0):
+    """Input gradient of gemm(x, w) = x w^T for the output gradient dy [.., M, N] (leading dims fold into M; row stride
+    allowed), read from the forward weight w [N, K] itself: dx [M, K] (+ residual [M, K]).  16-bit storage only."""
+    _ensure_workspace()
+    bf = _wgrad_storage(dy)
+    assert w.dtype == dy.dtype and dy.stride(-1) == 1 and w.dim() == 2 and w.stride(1) == 1
+    dy2 = _hp_rows(dy)
+    M, N = dy2.shape
+    K = w.shape[1]
+    assert w.shape[0] == N
+    if out is None:
+        out = torch.empty(M, K, device=dy.device, dtype=torch.float32 if out_f32 else dy.dtype)
+    assert out.dim() == 2 and tuple(out.shape) == (M, K) and out.stride(1) == 1
+    ld_res = 0
+    if residual is not None:
+        assert residual.dim() == 2 and residual.stride(1) == 1 and tuple(residual.shape) == (M, K)
+        ld_res = residual.stride(0)
+    e = _ep(None, None, 1, residual, ld_res, 0, alpha, out_scale, None, out.dtype == torch.float32)
+    check(lib().dm_gemm_dgrad(bf, ptr_any(dy2), dy2.stride(0), ptr_any(w), w.stride(0), ptr_any(out), out.stride(0), M, N, K,
+                              C.byref(e), bn, stream_ptr()), "dm_gemm_dgrad")
+    return out
+
+
 class Csd(C.Structure):
     _fields_ = [("noise", C.c_void_p), ("w", C.c_void_p), ("coef", C.c_void_p), ("grad", C.c_void_p),
                 ("dlatents", C.c_void_p), ("norms", C.c_void_p), ("eps_out", C.c_void_p)]
@@ -539,6 +590,31 @@ def silu(x):
     y = torch.empty_like(x)
     check(lib().dm_silu(bf, ptr_any(x), x.numel(), ptr_any(y), stream_ptr()), "dm_silu")
     return y
+
+
+def silu_bwd(z, dy):
+    """dy * silu'(z) on the pre-activation z.  16-bit storage only."""
+    bf = _is_bf16(z)    # fp32 storage: the library returns DM_EUNSUPPORTED
+    assert z.is_contiguous() and dy.is_contiguous() and dy.shape == z.shape and dy.dtype == z.dtype
+    dx = torch.empty_like(z)
+    check(lib().dm_silu_bwd(bf, ptr_any(z), ptr_any(dy), z.numel(), ptr_any(dx), stream_ptr()), "dm_silu_bwd")
+    return dx
+
+
+def rowvec_grad(dy, n_img, out=None):
+    """Gradient of the GEMM / conv epilogue's per-image `rowvec`: per-image column sums of dy [n_img * rows, N] (any leading
+    shape; a uniform row stride is allowed) -> [n_img, N] in the storage dtype, or into `out` (a column slice of a wider
+    buffer is fine).  16-bit storage only; deterministic."""
+    bf = _is_bf16(dy)
+    N = dy.shape[-1]
+    dy2 = dy.reshape(-1, N) if dy.is_contiguous() else _hp_rows(dy)
+    assert dy2.stride(1) == 1 and dy2.shape[0] % n_img == 0
+    if out is None:
+        out = torch.empty(n_img, N, device=dy.device, dtype=dy.dtype)
+    assert tuple(out.shape) == (n_img, N) and out.stride(1) == 1 and out.dtype == dy.dtype
+    check(lib().dm_rowvec_grad(bf, ptr_any(dy2), dy2.stride(0), n_img, dy2.shape[0] // n_img, N, ptr_any(out), out.stride(0),
+                               stream_ptr()), "dm_rowvec_grad")
+    return out
 
 
 def attention(q, k, v, heads, scale=None, out=None):

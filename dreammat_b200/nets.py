@@ -27,6 +27,7 @@ class _Base:
     def __init__(self, w: Dict[str, torch.Tensor], device, dtype):
         self.dev, self.dt = device, dtype
         self.p: Dict[str, torch.Tensor] = {}
+        self.conv_shape: Dict[str, tuple] = {}      # conv name -> diffusers [Cout, Cin, kh, kw] (before channel padding)
         self._src = w
 
     # ---- weight preparation
@@ -38,6 +39,7 @@ class _Base:
 
     def _conv(self, name, cin_pad=0, cout_pad=0):
         w = self._src[name + ".weight"]
+        self.conv_shape[name] = tuple(w.shape)
         self.p[name + ".w"] = D.conv_weight_to_gemm(w, cin_pad or _r64(w.shape[1]), cout_pad, self.dt).to(self.dev)
         if name + ".bias" in self._src:
             self._vec(name + ".bias", cout_pad)
@@ -125,28 +127,82 @@ class _UNetCommon(_Base):
         self._src = None  # drop the host copy
 
     # ---- forward pieces
-    def time_embed(self, t_f32):
-        """Timesteps -> TimestepEmbedding -> SiLU -> every resnet's time_emb_proj in one GEMM."""
+    def time_embed(self, t_f32, tape=None):
+        """Timesteps -> TimestepEmbedding -> SiLU -> every resnet's time_emb_proj in one GEMM.  With a tape (a dict) the
+        three GEMM inputs are recorded for time_embed_bwd."""
         P = self.p
-        e = D.timestep_embedding(t_f32, self.cfg.block_out_channels[0], self.dt)
-        e = D.gemm(e, P["time_embedding.linear_1.w"], bias=P["time_embedding.linear_1.bias"], act="silu")
+        e0 = D.timestep_embedding(t_f32, self.cfg.block_out_channels[0], self.dt)
+        e1 = D.gemm(e0, P["time_embedding.linear_1.w"], bias=P["time_embedding.linear_1.bias"], act="silu")
         # SiLU(temb) is the only consumer of temb (class embedding disabled, dreammat_guidance.py:311-317)
-        e = D.gemm(e, P["time_embedding.linear_2.w"], bias=P["time_embedding.linear_2.bias"], act="silu")
-        return D.gemm(e, P["tproj.w"], bias=P["tproj.b"])   # [N, sum Cout]
+        e2 = D.gemm(e1, P["time_embedding.linear_2.w"], bias=P["time_embedding.linear_2.bias"], act="silu")
+        if tape is not None:
+            tape.update(e0=e0, e1=e1, e2=e2)
+        return D.gemm(e2, P["tproj.w"], bias=P["tproj.b"])   # [N, sum Cout]
 
-    def resnet(self, p, x, tproj, out=None):
+    def time_embed_bwd(self, rec, d_tproj):
+        """Backward of time_embed(t, tape=rec) for d_tproj [N, sum Cout] (every resnet_bwd has written its columns):
+        gradients of tproj and both time_embedding linears.  The fused-SiLU GEMMs kept only their activated outputs, so
+        each pre-activation is recomputed by the same GEMM without the activation (M is the batch)."""
+        P, grads = self.p, {}
+        grads["tproj.w"], grads["tproj.b"] = D.gemm_wgrad(d_tproj, rec["e2"], bias=True)
+        d = D.gemm_dgrad(d_tproj, P["tproj.w"])
+        for name, xin in (("time_embedding.linear_2", rec["e1"]), ("time_embedding.linear_1", rec["e0"])):
+            z = D.gemm(xin, P[name + ".w"], bias=P[name + ".bias"])
+            dz = D.silu_bwd(z, d)
+            grads[name + ".w"], grads[name + ".bias"] = D.gemm_wgrad(dz, xin, bias=True)
+            if xin is not rec["e0"]:
+                d = D.gemm_dgrad(dz, P[name + ".w"])
+        return grads
+
+    def resnet(self, p, x, tproj, out=None, tape=None):
+        """ResnetBlock2D.  With a tape (a dict) it records what resnet_bwd needs: x, both GroupNorm statistics and conv1's
+        output; the activated GroupNorm outputs are recomputed in the backward rather than kept."""
         P, G = self.p, self.cfg.norm_groups
         n, H, W, Cin = x.shape
-        h, _ = D.groupnorm(x, P[p + ".norm1.weight"], P[p + ".norm1.bias"], G, 1e-5, silu=True)
+        h, st1 = D.groupnorm(x, P[p + ".norm1.weight"], P[p + ".norm1.bias"], G, 1e-5, silu=True)
         off, co = self.tproj_off[p]
-        h = D.conv2d(h, P[p + ".conv1.w"], 3, bias=P[p + ".conv1.bias"], rowvec=tproj[:, off:off + co])
-        h, _ = D.groupnorm(h, P[p + ".norm2.weight"], P[p + ".norm2.bias"], G, 1e-5, silu=True)
+        h1 = D.conv2d(h, P[p + ".conv1.w"], 3, bias=P[p + ".conv1.bias"], rowvec=tproj[:, off:off + co])
+        h, st2 = D.groupnorm(h1, P[p + ".norm2.weight"], P[p + ".norm2.bias"], G, 1e-5, silu=True)
+        xs = x if x.is_contiguous() else x.contiguous()
         if p + ".conv_shortcut.w" in P:
-            xs = x if x.is_contiguous() else x.contiguous()
             sc = D.gemm(xs.view(-1, Cin), P[p + ".conv_shortcut.w"], bias=P[p + ".conv_shortcut.bias"]).view(n, H, W, co)
         else:
             sc = x
+        if tape is not None:
+            tape.update(p=p, x=xs, st1=st1, h1=h1, st2=st2)
         return D.conv2d(h, P[p + ".conv2.w"], 3, bias=P[p + ".conv2.bias"], residual=sc, out=out)
+
+    def resnet_bwd(self, rec, dout, d_tproj, dx_add=None):
+        """Backward of resnet(p, x, tproj, tape=rec) for the output gradient dout [n, H, W, Cout]: returns (dx, grads) and
+        writes this resnet's columns of d_tproj [n, sum Cout].  dx_add is a second gradient of x (x also fed a skip
+        output): it rides on the shortcut's input-gradient GEMM as its residual, or costs one add when the shortcut is the
+        identity."""
+        P, G, p, x, h1 = self.p, self.cfg.norm_groups, rec["p"], rec["x"], rec["h1"]
+        n, H, W, Cin = x.shape
+        off, co = self.tproj_off[p]
+        g1, b1, g2, b2 = (P[p + k] for k in (".norm1.weight", ".norm1.bias", ".norm2.weight", ".norm2.bias"))
+        grads = {}
+        dout = dout if dout.is_contiguous() else dout.contiguous()
+        a2, _ = D.groupnorm(h1, g2, b2, G, 1e-5, silu=True)                      # conv2's input, recomputed
+        grads[p + ".conv2.w"], grads[p + ".conv2.bias"] = D.conv2d_wgrad(a2, dout, 3, bias=True)
+        da2 = D.conv2d_dgrad(dout, P[p + ".conv2.w"], 3)
+        dh1 = D.groupnorm_bwd(h1, da2, g2, b2, rec["st2"], G, 1e-5, silu=True)
+        grads[p + ".norm2.weight"], grads[p + ".norm2.bias"] = D.groupnorm_affine_grad(h1, da2, g2, b2, rec["st2"], G, silu=True)
+        D.rowvec_grad(dh1, n, out=d_tproj[:, off:off + co])
+        a1, _ = D.groupnorm(x, g1, b1, G, 1e-5, silu=True)                       # conv1's input, recomputed
+        grads[p + ".conv1.w"], grads[p + ".conv1.bias"] = D.conv2d_wgrad(a1, dh1, 3, bias=True)
+        da1 = D.conv2d_dgrad(dh1, P[p + ".conv1.w"], 3)
+        if p + ".conv_shortcut.w" in P:
+            grads[p + ".conv_shortcut.w"], grads[p + ".conv_shortcut.bias"] = D.gemm_wgrad(dout.view(-1, co), x.view(-1, Cin), bias=True)
+            dsc = D.gemm_dgrad(dout.view(-1, co), P[p + ".conv_shortcut.w"],
+                               residual=dx_add.view(-1, Cin) if dx_add is not None else None).view(n, H, W, Cin)
+        elif dx_add is not None:
+            dsc = D.axpby(dout.view(-1, co), 1.0, dx_add.view(-1, co), 1.0).view(n, H, W, co)
+        else:
+            dsc = dout
+        dx = D.groupnorm_bwd(x, da1, g1, b1, rec["st1"], G, 1e-5, silu=True, dx_add=dsc)
+        grads[p + ".norm1.weight"], grads[p + ".norm1.bias"] = D.groupnorm_affine_grad(x, da1, g1, b1, rec["st1"], G, silu=True)
+        return dx, grads
 
     def transformer(self, p, x, ctx, heads, tape=None):
         """Transformer2DModel (one BasicTransformerBlock).  With a tape (a dict) it also records what transformer_bwd
@@ -181,8 +237,8 @@ class _UNetCommon(_Base):
     def transformer_bwd(self, rec, dout):
         """Backward of transformer(p, x, ctx, heads, tape=rec) for the output gradient dout [n, H, W, C]: returns (dx,
         grads), grads mapping each prepared parameter name of the block to its fp32 gradient in the prepared layout (qkv /
-        kv fused, ff.net.0.proj value / gate interleaved).  ctx gets no gradient (the text encoder is frozen).  The dgrad
-        GEMMs use W^T built here from the current weights, and the GEGLU pre-activation is recomputed by one GEMM."""
+        kv fused, ff.net.0.proj value / gate interleaved).  ctx gets no gradient (the text encoder is frozen).  The input
+        gradients read the forward weights themselves (gemm_dgrad), and the GEGLU pre-activation is recomputed by one GEMM."""
         P, G, p, heads = self.p, self.cfg.norm_groups, rec["p"], rec["heads"]
         b = p + ".transformer_blocks.0"
         x = rec["x"]
@@ -195,7 +251,7 @@ class _UNetCommon(_Base):
             grads[name + ".w"] = dw
             if bias:
                 grads[name + ".bias"] = db
-            return D.gemm(dy.reshape(-1, dy.shape[-1]), D.transpose(P[name + ".w"]))
+            return D.gemm_dgrad(dy, P[name + ".w"])
 
         def ln(name, h, dn, dadd):
             dh, grads[name + ".weight"], grads[name + ".bias"] = D.layernorm_bwd(h, dn, P[name + ".weight"], dx_add=dadd)
@@ -228,24 +284,101 @@ class _UNetCommon(_Base):
         grads[p + ".norm.weight"], grads[p + ".norm.bias"] = D.groupnorm_affine_grad(x, dhN, gm, bt, rec["stats"], G)
         return dx, grads
 
-    def down_and_mid(self, sample, tproj, ctx):
+    def down_and_mid(self, sample, tproj, ctx, tape=None):
+        """Down blocks and mid block.  With a tape (a list) every resnet / transformer / downsampler appends one record;
+        a record whose input is also a skip output res[k] carries skip_in = k."""
         cfg = self.cfg
         res = [sample]
         n = len(cfg.block_out_channels)
+        skip = [0]                      # index of the skip output that the next layer consumes, or None
+
+        def rec(kind):
+            if tape is None:
+                return None
+            tape.append(dict(kind=kind, skip_in=skip[0]))
+            skip[0] = None
+            return tape[-1]
+
+        def push(s):
+            res.append(s)
+            skip[0] = len(res) - 1
+
         for i in range(n):
             for j in range(cfg.layers_per_block):
-                sample = self.resnet(f"down_blocks.{i}.resnets.{j}", sample, tproj)
+                sample = self.resnet(f"down_blocks.{i}.resnets.{j}", sample, tproj, tape=rec("resnet"))
                 if i < n - 1:
-                    sample = self.transformer(f"down_blocks.{i}.attentions.{j}", sample, ctx, cfg.heads[i])
-                res.append(sample)
+                    sample = self.transformer(f"down_blocks.{i}.attentions.{j}", sample, ctx, cfg.heads[i], tape=rec("transformer"))
+                push(sample)
             if i < n - 1:
                 pn = f"down_blocks.{i}.downsamplers.0.conv"
+                r = rec("down")
+                if r is not None:
+                    r.update(p=pn, x=sample)
                 sample = D.conv2d(sample, self.p[pn + ".w"], 3, stride=2, pad=(1, 1), bias=self.p[pn + ".bias"])
-                res.append(sample)
-        sample = self.resnet("mid_block.resnets.0", sample, tproj)
-        sample = self.transformer("mid_block.attentions.0", sample, ctx, cfg.heads[-1])
-        sample = self.resnet("mid_block.resnets.1", sample, tproj)
+                push(sample)
+        sample = self.resnet("mid_block.resnets.0", sample, tproj, tape=rec("resnet"))
+        sample = self.transformer("mid_block.attentions.0", sample, ctx, cfg.heads[-1], tape=rec("transformer"))
+        sample = self.resnet("mid_block.resnets.1", sample, tproj, tape=rec("resnet"))
         return res, sample
+
+    def down_and_mid_bwd(self, tape, d_res, d_mid, d_tproj):
+        """Backward of down_and_mid(sample, tproj, ctx, tape=tape): d_res[k] is the gradient of skip output res[k] (None
+        for none), d_mid that of the mid block's output.  Walks the tape in reverse; returns (d_sample, grads) with d_res[0]
+        included in d_sample, and fills d_tproj.  Where an activation feeds a skip output and the next layer, the skip's
+        gradient is the residual of that layer's input-gradient kernel (downsampler, resnet with a shortcut) or one add
+        (resnet whose shortcut is the identity)."""
+        grads = {}
+        d = d_mid
+        for r in reversed(tape):
+            extra = d_res[r["skip_in"]] if r["skip_in"] is not None else None
+            if r["kind"] == "resnet":
+                d, g = self.resnet_bwd(r, d, d_tproj, dx_add=extra)
+            elif r["kind"] == "transformer":
+                assert extra is None      # a transformer's input is a resnet's output, never a skip output
+                d, g = self.transformer_bwd(r, d)
+            else:
+                pn = r["p"]
+                d = d if d.is_contiguous() else d.contiguous()
+                g = {}
+                g[pn + ".w"], g[pn + ".bias"] = D.conv2d_wgrad(r["x"], d, 3, stride=2, pad=(1, 1), bias=True)
+                d = D.conv2d_dgrad(D.upsample2x(d, zero_insert=True), self.p[pn + ".w"], 3, pad=(1, 1), residual=extra)
+            grads.update(g)
+        return d, grads
+
+    def grads_to_state_dict(self, grads):
+        """Prepared-layout gradients -> diffusers state-dict names and shapes (what a checkpoint or a stock optimizer
+        consumes): convolutions back to [Cout, Cin, kh, kw] with the channel padding dropped, q / k / v split, the GEGLU
+        projection de-interleaved, time_emb_proj un-stacked."""
+        out = {}
+        for k, v in grads.items():
+            base = k.rsplit(".", 1)[0]
+            if base in self.conv_shape:
+                co, ci, kh, kw = self.conv_shape[base]
+                if k.endswith(".w"):
+                    out[base + ".weight"] = v.view(v.shape[0], kh, kw, -1)[:co, :, :, :ci].permute(0, 3, 1, 2).contiguous()
+                else:
+                    out[k] = v[:co]
+            elif k in ("tproj.w", "tproj.b"):
+                for p, (off, co) in self.tproj_off.items():
+                    out[p + (".time_emb_proj.weight" if k == "tproj.w" else ".time_emb_proj.bias")] = v[off:off + co]
+            elif k.endswith(".attn1.qkv.w"):
+                C = v.shape[0] // 3
+                for i, nm in enumerate(("to_q", "to_k", "to_v")):
+                    out[f"{base[:-4]}.{nm}.weight"] = v[i * C:(i + 1) * C]
+            elif k.endswith(".attn2.kv.w"):
+                C = v.shape[0] // 2
+                out[base[:-3] + ".to_k.weight"], out[base[:-3] + ".to_v.weight"] = v[:C], v[C:]
+            elif base.endswith(".ff.net.0.proj"):
+                D2 = v.shape[0] // 2                       # interleaved blocks of 32 value rows, then 32 gate rows
+                blk = v.reshape(D2 // 32, 2, 32, *v.shape[1:])
+                out[base + (".weight" if k.endswith(".w") else ".bias")] = torch.cat(
+                    [blk[:, 0].reshape(D2, *v.shape[1:]), blk[:, 1].reshape(D2, *v.shape[1:])], 0)
+            elif k.endswith(".w"):
+                is_1x1 = base.endswith(".conv_shortcut") or base.startswith("controlnet_")
+                out[base + ".weight"] = v[:, :, None, None] if is_1x1 else v
+            else:
+                out[k] = v
+        return out
 
 
 class UNet(_UNetCommon):
@@ -327,20 +460,44 @@ class ControlNet(_UNetCommon):
         self._vec("controlnet_mid_block.bias")
         self._finish_tproj()
 
-    def cond_embed(self, cond_nhwc):
-        """ControlNetConditioningEmbedding: cond [B,8h,8w,64] (22 real channels) -> [B,h,w,C0]."""
+    def cond_embed(self, cond_nhwc, tape=None):
+        """ControlNetConditioningEmbedding: cond [B,8h,8w,64] (22 real channels) -> [B,h,w,C0].  With a tape (a list) the
+        input of every convolution is recorded for cond_embed_bwd."""
         P = self.p
-        c = D.conv2d(cond_nhwc, P["controlnet_cond_embedding.conv_in.w"], 3, bias=P["controlnet_cond_embedding.conv_in.bias"], act="silu")
+        pe = "controlnet_cond_embedding."
         nb = 2 * (len(self.cfg.cond_embed_channels) - 1)
-        for i in range(nb):
-            pn = f"controlnet_cond_embedding.blocks.{i}"
-            c = D.conv2d(c, P[pn + ".w"], 3, stride=2 if i % 2 == 1 else 1, pad=(1, 1), bias=P[pn + ".bias"], act="silu")
-        return D.conv2d(c, P["controlnet_cond_embedding.conv_out.w"], 3, bias=P["controlnet_cond_embedding.conv_out.bias"])
+        layers = [(pe + "conv_in", 1, "silu")] + [(f"{pe}blocks.{i}", 1 + i % 2, "silu") for i in range(nb)] + [(pe + "conv_out", 1, None)]
+        c = cond_nhwc
+        for pn, stride, act in layers:
+            if tape is not None:
+                tape.append((pn, stride, act, c))
+            c = D.conv2d(c, P[pn + ".w"], 3, stride=stride, pad=(1, 1), bias=P[pn + ".bias"], act=act)
+        return c
 
-    def forward(self, sample_nhwc, t_f32, ctx, cond_nhwc, conditioning_scale=1.0):
+    def cond_embed_bwd(self, tape, dc):
+        """Backward of cond_embed(cond, tape=tape) for the embedding's gradient dc: gradients of its eight convolutions (the
+        condition itself gets none).  The forward fuses SiLU into the convolution and keeps only the activated output, so
+        each pre-activation is recomputed by the same convolution without the activation.  Padded channels (22 -> 64
+        condition, 16 / 32 / 96 -> 64 / 64 / 128 widths) carry zero activations and zero weights, so their gradients come
+        out exactly zero."""
+        P, grads = self.p, {}
+        d = dc if dc.is_contiguous() else dc.contiguous()
+        for k, (pn, stride, act, x) in reversed(list(enumerate(tape))):
+            if act is not None:
+                z = D.conv2d(x, P[pn + ".w"], 3, stride=stride, pad=(1, 1), bias=P[pn + ".bias"])
+                d = D.silu_bwd(z, d)
+            grads[pn + ".w"], grads[pn + ".bias"] = D.conv2d_wgrad(x, d, 3, stride=stride, pad=(1, 1), bias=True)
+            if k > 0:
+                d = D.conv2d_dgrad(D.upsample2x(d, zero_insert=True) if stride == 2 else d, P[pn + ".w"], 3, pad=(1, 1))
+        return grads
+
+    def forward(self, sample_nhwc, t_f32, ctx, cond_nhwc, conditioning_scale=1.0, tape=None):
+        """Returns (down residuals, mid residual).  With a tape (a dict) it also records what backward() needs; the outputs
+        are the same bits either way."""
         P = self.p
-        tproj = self.time_embed(t_f32)
-        c = self.cond_embed(cond_nhwc)
+        rec = tape is not None
+        tproj = self.time_embed(t_f32, tape=tape.setdefault("time", {}) if rec else None)
+        c = self.cond_embed(cond_nhwc, tape=tape.setdefault("cond", []) if rec else None)
         N_ = sample_nhwc.shape[0]
         B = c.shape[0]
         rep = N_ // B
@@ -348,7 +505,10 @@ class ControlNet(_UNetCommon):
         for k in range(rep):   # the embedding of view b is shared by its CFG branches (layout [branch][view])
             D.axpby(c.view(-1, c.shape[-1]), 1.0, out=c_rep[k * B:(k + 1) * B].view(-1, c.shape[-1]))
         sample = D.conv2d(sample_nhwc, P["conv_in.w"], 3, bias=P["conv_in.bias"], residual=c_rep)
-        res, mid = self.down_and_mid(sample, tproj, ctx)
+        res, mid = self.down_and_mid(sample, tproj, ctx, tape=tape.setdefault("walk", []) if rec else None)
+        if rec:
+            res = [r if r.is_contiguous() else r.contiguous() for r in res]
+            tape.update(sample_in=sample_nhwc, res=res, mid=mid, scale=conditioning_scale, n_cond=B, tproj_shape=tproj.shape)
         down = []
         for i, r in enumerate(res):
             n, H, W, C = r.shape
@@ -359,6 +519,36 @@ class ControlNet(_UNetCommon):
         mid = D.gemm(mid.view(-1, C), P["controlnet_mid_block.w"], bias=P["controlnet_mid_block.bias"],
                      out_scale=conditioning_scale).view(n, H, W, C)
         return down, mid
+
+    def backward(self, tape, d_down, d_mid):
+        """Gradients of every parameter from the gradients of forward(..., tape=tape)'s fourteen outputs: d_down[i] / d_mid
+        in the outputs' shapes and storage type.  Returns grads mapping EVERY key of self.p to an fp32 tensor in that key's
+        prepared layout (grads_to_state_dict maps them to diffusers names).  The noisy latents, the condition, the
+        timesteps and ctx get no gradient."""
+        P, scale = self.p, tape["scale"]
+        grads = {}
+
+        def zero_conv(name, dy, r):
+            C = r.shape[-1]
+            dy = dy.reshape(-1, C) if dy.is_contiguous() else dy.contiguous().view(-1, C)
+            if scale != 1.0:      # out = scale * (W r + b): fold the scale into the gradient once
+                dy = D.axpby(dy, scale)
+            grads[name + ".w"], grads[name + ".bias"] = D.gemm_wgrad(dy, r.view(-1, C), bias=True)
+            return D.gemm_dgrad(dy, P[name + ".w"]).view(r.shape)
+
+        d_res = [zero_conv(f"controlnet_down_blocks.{i}", d_down[i], r) for i, r in enumerate(tape["res"])]
+        d_m = zero_conv("controlnet_mid_block", d_mid, tape["mid"])
+        d_tproj = torch.empty(tape["tproj_shape"], device=self.dev, dtype=self.dt)
+        d_sample, g = self.down_and_mid_bwd(tape["walk"], d_res, d_m, d_tproj)
+        grads.update(g)
+        grads["conv_in.w"], grads["conv_in.bias"] = D.conv2d_wgrad(tape["sample_in"], d_sample, 3, bias=True)
+        B = tape["n_cond"]
+        dc = d_sample[:B]             # the embedding is shared by the rep copies of a view: its gradient is their sum
+        for k in range(1, d_sample.shape[0] // B):
+            dc = D.axpby(dc.reshape(-1, dc.shape[-1]), 1.0, d_sample[k * B:(k + 1) * B].view(-1, dc.shape[-1]), 1.0).view(dc.shape)
+        grads.update(self.cond_embed_bwd(tape["cond"], dc))
+        grads.update(self.time_embed_bwd(tape["time"], d_tproj))
+        return grads
 
 
 # ================================================================================================ VAE encoder

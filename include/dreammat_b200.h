@@ -17,11 +17,12 @@
  * a summation order).  Still accumulated with fp32 atomics: the logged sums (norms of dm_conv2d_csd / dm_sds_grad, reg_sums
  * of the shading) and the adjoint of dm_resize_bilinear (renders that are not 512^2).  Weight gradients (dm_conv2d_wgrad /
  * dm_gemm_wgrad) sum each element in one fixed K order, split-K slices in slice order, and the bias gradient's per-block
- * partial rows in row order.  dm_attention_bwd gives every dQ / dK / dV element to one CTA, which sums its blocks in
+ * partial rows in row order.  Input gradients (dm_conv2d_dgrad / dm_gemm_dgrad) are the forward kernel: one fixed K order per
+ * element, split-K slices in slice order.  dm_attention_bwd gives every dQ / dK / dV element to one CTA, which sums its blocks in
  * order (S and dP are recomputed rather than dQ added atomically); its delta scratch comes from the caller.  dm_groupnorm / dm_groupnorm_bwd (per-block partial sums), the bias gradient of
  * dm_conv2d_wgrad / dm_gemm_wgrad (per-block partial rows), dm_antialias_fwd / _bwd (per-pixel pair buckets) and
  * dm_hashgrid_mlp_bwd (int64 fixed-point grid gradient), dm_layernorm_bwd / dm_groupnorm_affine_grad (per-chunk partial
- * rows of the affine gradients) need scratch for that which their signatures have no room for; the library allocates it once per device, on
+ * rows of the affine gradients) and dm_rowvec_grad (per-chunk partial rows, the same slot) need scratch for that which their signatures have no room for; the library allocates it once per device, on
  * the first call (not while the stream is being captured: run a call once before capturing it), and never frees it.  Calls
  * on one device must not run concurrently on two streams.
  */
@@ -251,6 +252,26 @@ int dm_conv2d_wgrad(int bf16, const void* x, int n_img, int H, int W, int Cin, c
  * x [M, ldx]; K % 64 == 0; M arbitrary (>= 1).  Deterministic. */
 int dm_gemm_wgrad(int bf16, const void* dy, int64_t ld_dy, const void* x, int64_t ldx, int M, int N, int K, float* dw,
                   float* db, void* stream);
+/* Input gradients (the `input.grad` autograd computes for a conv / linear layer), read straight from the FORWARD weight: no
+ * flipped / transposed copy, so they follow a weight that an optimizer updates in place.  The same tensor-core kernel as
+ * the forward, with the weight as its MN-major operand: the tap flip of the transposed convolution is a TMA coordinate.
+ * Planned as the contraction [M = pixels (tokens), N = Cin (K_in), K = k*k*Cout (N_out)]: dm_gemm_plan(M, N, K, act,
+ * bn_hint, ...) reports the tile and split-K a call uses.  The whole dm_epilogue applies (`residual` adds a second gradient
+ * branch in the same kernel, alpha / out_scale scale it; act 3 is rejected); dx is 16-bit, or fp32 with out_f32.  The K
+ * order and every product are those of dm_conv2d on conv_weight_to_gemm(W.flip(2,3).permute(1,0,2,3)) and of dm_gemm on
+ * W^T, so the results are bit-identical to those.  16-bit storage only: bf16 == 2 returns DM_EUNSUPPORTED.  Bad shapes,
+ * strides or alignment return DM_EINVAL before any launch.  Deterministic.
+ *
+ * dx[n,H,W,ldc] (first Cin channels) = d/dx of the stride-1 dm_conv2d(x, w, ksize, pad_t, pad_l) . dy, for dy [n,H,W,Cout]
+ * dense (Cout % 64 == 0: it is the reduction axis) and w [Cout, k*k*Cin] the forward's weight (Cin % 8 == 0).  pad_t / pad_l
+ * are those of the FORWARD convolution (the kernel shifts by k-1-pad).  A stride-2 forward is differentiated by
+ * dm_upsample2x(zero_insert=1) on dy followed by this call. */
+int dm_conv2d_dgrad(int bf16, const void* dy, int n_img, int H, int W, int Cout, const void* w, int Cin, int ksize,
+                    int pad_t, int pad_l, void* dx, int64_t ldc, const dm_epilogue* ep, int bn_hint, void* stream);
+/* dx[M, ldc] (first K_in columns) = dy[M, N_out] . w[N_out, K_in]; dy row stride ld_dy, w row stride ldw (the forward's
+ * weight; a row slice of a fused projection is fine).  N_out % 64 == 0, K_in % 8 == 0, M arbitrary (>= 1). */
+int dm_gemm_dgrad(int bf16, const void* dy, int64_t ld_dy, const void* w, int64_t ldw, void* dx, int64_t ldc, int M,
+                  int N_out, int K_in, const dm_epilogue* ep, int bn_hint, void* stream);
 
 /* conv_out of the UNet with the CSD / SDS combination fused into its epilogue: the model-level tail of
  * `dm_unet_fwd_sds` (SURVEY.md section 8b).  Replaces conv_out (dreammat_guidance.py:274-282), the `.sample` layout /
@@ -351,6 +372,15 @@ int dm_add_noise(int bf16, const float* z, const float* noise, const float* sqrt
                  int HW, int cpad, int rep, void* out, void* stream);
 int dm_timestep_embedding(int bf16, const float* t, int n, int dim, void* out, void* stream);
 int dm_silu(int bf16, const void* x, int64_t n, void* y, void* stream);
+/* dx = dy * silu'(z) on the pre-activation z (backward of a SiLU epilogue); n % 8 == 0, 16-byte aligned operands; 16-bit
+ * only (bf16 == 2: DM_EUNSUPPORTED). */
+int dm_silu_bwd(int bf16, const void* z, const void* dy, int64_t n, void* dx, void* stream);
+/* Gradient of dm_epilogue.rowvec (a resnet's slice of the time-embedding projection): out[img, c] = sum over the image's
+ * rows of dy[img*rows_per_img + r, c], c < N, in the storage dtype (fp32 accumulation).  dy [n_img*rows_per_img, ld], out
+ * [n_img, ld_out], so out can be a column slice of a wider gradient buffer.  N % 8 == 0, ld % 8 == 0.  Per-chunk partial
+ * rows (library scratch, see DETERMINISM) are added in chunk order.  16-bit only (bf16 == 2: DM_EUNSUPPORTED). */
+int dm_rowvec_grad(int bf16, const void* dy, int64_t ld, int n_img, int rows_per_img, int N, void* out, int64_t ld_out,
+                   void* stream);
 
 /* Fused attention, head_dim 64: O = softmax(scale * Q K^T) V per (batch, head).  Q [batch,Nq,ldq],
  * K/V [batch,Nk,ldkv], O [batch,Nq,ldo]; head h occupies columns [64h, 64h+64) of every operand.
