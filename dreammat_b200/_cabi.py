@@ -112,6 +112,8 @@ SIGNATURES = {
     "dm_gemm_dgrad": (C.c_int, [C.c_int, P, I64, P, I64, P, I64, C.c_int, C.c_int, C.c_int, P, C.c_int, P]),
     "dm_silu_bwd": (C.c_int, [C.c_int, P, P, I64, P, P]),
     "dm_rowvec_grad": (C.c_int, [C.c_int, P, I64, C.c_int, C.c_int, C.c_int, P, I64, P]),
+    "dm_upsample2x_bwd": (C.c_int, [C.c_int, P] + [C.c_int] * 4 + [P, P]),
+    "dm_mse_loss_grad": (C.c_int, [C.c_int, P, P, C.c_int, C.c_int, C.c_int, F, P, C.c_int, P, P]),
 }
 
 

@@ -762,6 +762,95 @@ __global__ void __launch_bounds__(256) rowvec_finish_kernel(const float* __restr
     out[img * ld_out + c] = H<T>::t(s);
 }
 
+// Adjoint of the nearest 2x upsample: dx[img, y, x, :] = the sum of dy's 2x2 block (2y + a, 2x + b), added in the order
+// (0,0), (0,1), (1,0), (1,1) in fp32 and rounded once.  A thread owns one 8-channel vector of dx.
+template <typename T>
+__global__ void __launch_bounds__(256) upsample2x_bwd_kernel(const T* __restrict__ dy, int n, int Hh, int W, int C,
+                                                             T* __restrict__ dx) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int64_t nv = (int64_t)n * Hh * W * (C / 8);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i % (C / 8)); int64_t r = i / (C / 8);
+        const int xo = (int)(r % W); r /= W;
+        const int yo = (int)(r % Hh); const int img = (int)(r / Hh);
+        const T* src = dy + (((int64_t)img * 2 * Hh + 2 * yo) * 2 * W + 2 * xo) * C + 8 * c;
+        const int64_t row = (int64_t)2 * W * C;
+        const uint4 u[4] = {*reinterpret_cast<const uint4*>(src), *reinterpret_cast<const uint4*>(src + C),
+                            *reinterpret_cast<const uint4*>(src + row), *reinterpret_cast<const uint4*>(src + row + C)};
+        float s[8] = {};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const T* h = reinterpret_cast<const T*>(&u[q]);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) s[k] += H<T>::f(h[k]);
+        }
+        uint4 o; T* oh = reinterpret_cast<T*>(&o);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) oh[k] = H<T>::t(s[k]);
+        reinterpret_cast<uint4*>(dx)[i] = o;
+    }
+}
+
+// Gradient of F.mse_loss(pred, target) (mean reduction) for pred / target fp32 NCHW [n, C, HW]: a thread owns pixels q of
+// the grid-stride loop, reads its C channels (coalesced along HW), writes the pixel's whole NHWC row of d_pred [n*HW, ld]
+// (coef * (pred - target) for c < C, zero for the padding channels) and adds (pred - target)^2 to its fp32 sum.  Each
+// block reduces its threads in a fixed order into part[block]; mse_loss_finish_kernel adds the rows in block order.
+template <typename T>
+__global__ void __launch_bounds__(256) mse_loss_grad_kernel(const float* __restrict__ pred, const float* __restrict__ target,
+                                                            int C, int HW, int64_t npix, int ld, float coef,
+                                                            T* __restrict__ d_pred, float* __restrict__ part) {
+    griddep_launch_dependents();
+    griddep_wait();
+    float acc = 0.f;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < npix; q += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t img = q / HW, p = q - img * HW;
+        const float* pp = pred + img * C * HW + p;
+        const float* tp = target + img * C * HW + p;
+        uint4* drow = reinterpret_cast<uint4*>(d_pred + q * ld);
+        for (int v = 0; v < ld / 8; ++v) {
+            uint4 o; T* oh = reinterpret_cast<T*>(&o);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const int c = 8 * v + k;
+                oh[k] = H<T>::t(0.f);
+                if (c < C) {
+                    const float d = pp[(int64_t)c * HW] - tp[(int64_t)c * HW];
+                    acc += d * d;
+                    oh[k] = H<T>::t(coef * d);
+                }
+            }
+            drow[v] = o;
+        }
+    }
+    __shared__ float red[8];
+    acc = warp_sum(acc);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float s = 0.f;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += red[w];
+        part[blockIdx.x] = s;
+    }
+}
+
+__global__ void __launch_bounds__(256) mse_loss_finish_kernel(const float* __restrict__ part, int nblk, float inv_numel,
+                                                              float* __restrict__ loss) {
+    griddep_launch_dependents();
+    griddep_wait();
+    float s = 0.f;
+    for (int b = threadIdx.x; b < nblk; b += blockDim.x) s += part[b];
+    __shared__ float red[8];
+    s = warp_sum(s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = 0.f;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
+        *loss = t * inv_numel;
+    }
+}
+
 // ----------------------------------------------------------------------------------- norm / GEGLU backward
 // LayerNorm backward, warp per row (the forward's mapping): mean / rstd recomputed from x with the forward's arithmetic,
 // g = dy * gamma, dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dx_add).  (mean, rstd) of each row go to `rstats`
@@ -1190,6 +1279,42 @@ extern "C" int dm_rowvec_grad(int bf16, const void* dy, int64_t ld, int n_img, i
     DM_CHECK_LAUNCH();
     DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(rowvec_finish_kernel<T>, dim3((unsigned)dm_ceil_div((int64_t)n_img * N, 256)), dim3(256), 0, st,
                                                 (const float*)part, chunks, N, n_img, (T*)out, ld_out)));
+    DM_CHECK_LAUNCH();
+    return DM_OK;
+}
+
+extern "C" int dm_upsample2x_bwd(int bf16, const void* dy, int n, int H, int W, int C, void* dx, void* stream) {
+    DM_DTYPE_OK(bf16);
+    if (bf16 == 2) { dm_set_error("dm_upsample2x_bwd: fp32 storage is not supported (16-bit only)"); return DM_EUNSUPPORTED; }
+    DM_REQUIRE(dy && dx, "null pointer");
+    DM_REQUIRE(n > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "positive extents, C a multiple of 8");
+    DM_REQUIRE((((uintptr_t)dy | (uintptr_t)dx) & 15) == 0, "16-byte aligned operands");
+    const int64_t nv = (int64_t)n * H * W * (C / 8);
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(upsample2x_bwd_kernel<T>, dim3((unsigned)grid_for(nv)), dim3(256), 0, (cudaStream_t)stream,
+                                                (const T*)dy, n, H, W, C, (T*)dx)));
+    DM_CHECK_LAUNCH();
+    return DM_OK;
+}
+
+extern "C" int dm_mse_loss_grad(int bf16, const float* pred, const float* target, int n, int C, int HW, float grad_scale,
+                                void* d_pred, int ld_d, float* loss, void* stream) {
+    DM_DTYPE_OK(bf16);
+    if (bf16 == 2) { dm_set_error("dm_mse_loss_grad: fp32 storage is not supported (16-bit only)"); return DM_EUNSUPPORTED; }
+    DM_REQUIRE(pred && target && d_pred && loss, "null pointer");
+    DM_REQUIRE(n > 0 && C > 0 && HW > 0, "positive extents");
+    DM_REQUIRE(ld_d % 64 == 0 && ld_d >= C, "d_pred row stride a multiple of 64 channels, at least C");
+    DM_REQUIRE(((uintptr_t)d_pred & 15) == 0 && (((uintptr_t)pred | (uintptr_t)target | (uintptr_t)loss) & 3) == 0,
+               "d_pred 16-byte aligned, pred / target / loss 4-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t npix = (int64_t)n * HW;
+    const double numel = (double)npix * C;
+    const int nblk = grid_for(npix);
+    float* part = (float*)dm_scratch(DM_SCRATCH_AFFINE, (size_t)nblk * sizeof(float), st);
+    if (!part) return DM_EDRIVER;
+    DM_DISPATCH_T(bf16, DM_CHECK_CUDA(dm_launch(mse_loss_grad_kernel<T>, dim3((unsigned)nblk), dim3(256), 0, st, pred, target, C, HW,
+                                                npix, ld_d, (float)(grad_scale * 2.0 / numel), (T*)d_pred, part)));
+    DM_CHECK_LAUNCH();
+    DM_CHECK_CUDA(dm_launch(mse_loss_finish_kernel, dim3(1), dim3(256), 0, st, (const float*)part, nblk, (float)(1.0 / numel), loss));
     DM_CHECK_LAUNCH();
     return DM_OK;
 }

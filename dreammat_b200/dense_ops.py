@@ -456,6 +456,32 @@ def upsample2x(x, zero_insert=False):
     return y
 
 
+def upsample2x_bwd(dy):
+    """Adjoint of upsample2x(x) (nearest): dy [n, 2H, 2W, C] -> dx [n, H, W, C], the sum of each 2x2 block (fp32, rounded
+    once).  16-bit storage only."""
+    bf = _is_bf16(dy)    # fp32 storage: the library returns DM_EUNSUPPORTED
+    assert dy.is_contiguous()
+    n, H2, W2, Cc = dy.shape
+    assert H2 % 2 == 0 and W2 % 2 == 0
+    dx = torch.empty(n, H2 // 2, W2 // 2, Cc, device=dy.device, dtype=dy.dtype)
+    check(lib().dm_upsample2x_bwd(bf, ptr_any(dy), n, H2 // 2, W2 // 2, Cc, ptr_any(dx), stream_ptr()), "dm_upsample2x_bwd")
+    return dx
+
+
+def mse_loss_grad(pred, target, dtype, ld=64, grad_scale=1.0):
+    """F.mse_loss(pred, target) and its gradient: pred / target fp32 NCHW [n, C, H, W] -> (loss, d_pred), loss a 0-dim fp32
+    device tensor (unscaled), d_pred NHWC [n, H, W, ld] in `dtype` = grad_scale * d loss / d pred, its padding channels
+    zero, ready for conv2d_dgrad.  16-bit storage only; deterministic, no host synchronisation."""
+    assert pred.dtype == torch.float32 and target.dtype == torch.float32 and pred.shape == target.shape and pred.dim() == 4
+    assert pred.is_contiguous() and target.is_contiguous()
+    n, Cc, H, W = pred.shape
+    loss = torch.empty((), device=pred.device, dtype=torch.float32)
+    d_pred = torch.empty(n, H, W, ld, device=pred.device, dtype=dtype)
+    check(lib().dm_mse_loss_grad(_dt_code(dtype), ptr_any(pred), ptr_any(target), n, Cc, H * W, grad_scale, ptr_any(d_pred), ld,
+                                 ptr_any(loss), stream_ptr()), "dm_mse_loss_grad")
+    return loss, d_pred
+
+
 def axpby(s1, a=1.0, s2=None, b=1.0, out=None):
     """out[..., :] = a*s1 + b*s2 over 2-D views [rows, cols] with arbitrary row strides (last dim contiguous)."""
     bf = _is_bf16(s1)

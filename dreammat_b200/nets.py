@@ -172,28 +172,32 @@ class _UNetCommon(_Base):
             tape.update(p=p, x=xs, st1=st1, h1=h1, st2=st2)
         return D.conv2d(h, P[p + ".conv2.w"], 3, bias=P[p + ".conv2.bias"], residual=sc, out=out)
 
-    def resnet_bwd(self, rec, dout, d_tproj, dx_add=None):
+    def resnet_bwd(self, rec, dout, d_tproj, dx_add=None, params=True):
         """Backward of resnet(p, x, tproj, tape=rec) for the output gradient dout [n, H, W, Cout]: returns (dx, grads) and
         writes this resnet's columns of d_tproj [n, sum Cout].  dx_add is a second gradient of x (x also fed a skip
         output): it rides on the shortcut's input-gradient GEMM as its residual, or costs one add when the shortcut is the
-        identity."""
+        identity.  params=False computes dx alone (a frozen block): no parameter or d_tproj gradient (d_tproj may be None),
+        and none of the GroupNorm recomputations that only feed them; grads is then empty."""
         P, G, p, x, h1 = self.p, self.cfg.norm_groups, rec["p"], rec["x"], rec["h1"]
         n, H, W, Cin = x.shape
         off, co = self.tproj_off[p]
         g1, b1, g2, b2 = (P[p + k] for k in (".norm1.weight", ".norm1.bias", ".norm2.weight", ".norm2.bias"))
         grads = {}
         dout = dout if dout.is_contiguous() else dout.contiguous()
-        a2, _ = D.groupnorm(h1, g2, b2, G, 1e-5, silu=True)                      # conv2's input, recomputed
-        grads[p + ".conv2.w"], grads[p + ".conv2.bias"] = D.conv2d_wgrad(a2, dout, 3, bias=True)
+        if params:
+            a2, _ = D.groupnorm(h1, g2, b2, G, 1e-5, silu=True)                  # conv2's input, recomputed
+            grads[p + ".conv2.w"], grads[p + ".conv2.bias"] = D.conv2d_wgrad(a2, dout, 3, bias=True)
         da2 = D.conv2d_dgrad(dout, P[p + ".conv2.w"], 3)
         dh1 = D.groupnorm_bwd(h1, da2, g2, b2, rec["st2"], G, 1e-5, silu=True)
-        grads[p + ".norm2.weight"], grads[p + ".norm2.bias"] = D.groupnorm_affine_grad(h1, da2, g2, b2, rec["st2"], G, silu=True)
-        D.rowvec_grad(dh1, n, out=d_tproj[:, off:off + co])
-        a1, _ = D.groupnorm(x, g1, b1, G, 1e-5, silu=True)                       # conv1's input, recomputed
-        grads[p + ".conv1.w"], grads[p + ".conv1.bias"] = D.conv2d_wgrad(a1, dh1, 3, bias=True)
+        if params:
+            grads[p + ".norm2.weight"], grads[p + ".norm2.bias"] = D.groupnorm_affine_grad(h1, da2, g2, b2, rec["st2"], G, silu=True)
+            D.rowvec_grad(dh1, n, out=d_tproj[:, off:off + co])
+            a1, _ = D.groupnorm(x, g1, b1, G, 1e-5, silu=True)                   # conv1's input, recomputed
+            grads[p + ".conv1.w"], grads[p + ".conv1.bias"] = D.conv2d_wgrad(a1, dh1, 3, bias=True)
         da1 = D.conv2d_dgrad(dh1, P[p + ".conv1.w"], 3)
         if p + ".conv_shortcut.w" in P:
-            grads[p + ".conv_shortcut.w"], grads[p + ".conv_shortcut.bias"] = D.gemm_wgrad(dout.view(-1, co), x.view(-1, Cin), bias=True)
+            if params:
+                grads[p + ".conv_shortcut.w"], grads[p + ".conv_shortcut.bias"] = D.gemm_wgrad(dout.view(-1, co), x.view(-1, Cin), bias=True)
             dsc = D.gemm_dgrad(dout.view(-1, co), P[p + ".conv_shortcut.w"],
                                residual=dx_add.view(-1, Cin) if dx_add is not None else None).view(n, H, W, Cin)
         elif dx_add is not None:
@@ -201,7 +205,8 @@ class _UNetCommon(_Base):
         else:
             dsc = dout
         dx = D.groupnorm_bwd(x, da1, g1, b1, rec["st1"], G, 1e-5, silu=True, dx_add=dsc)
-        grads[p + ".norm1.weight"], grads[p + ".norm1.bias"] = D.groupnorm_affine_grad(x, da1, g1, b1, rec["st1"], G, silu=True)
+        if params:
+            grads[p + ".norm1.weight"], grads[p + ".norm1.bias"] = D.groupnorm_affine_grad(x, da1, g1, b1, rec["st1"], G, silu=True)
         return dx, grads
 
     def transformer(self, p, x, ctx, heads, tape=None):
@@ -234,11 +239,13 @@ class _UNetCommon(_Base):
                         n2=n2, q=q, kv=kv, o2=o2, lse2=lse2, h2=h2, n3=n3, f=f, h3=h3)
         return D.gemm(h3, P[p + ".proj_out.w"], bias=P[p + ".proj_out.bias"], residual=xs.view(M, C)).view(n, H, W, C)
 
-    def transformer_bwd(self, rec, dout):
+    def transformer_bwd(self, rec, dout, params=True):
         """Backward of transformer(p, x, ctx, heads, tape=rec) for the output gradient dout [n, H, W, C]: returns (dx,
         grads), grads mapping each prepared parameter name of the block to its fp32 gradient in the prepared layout (qkv /
         kv fused, ff.net.0.proj value / gate interleaved).  ctx gets no gradient (the text encoder is frozen).  The input
-        gradients read the forward weights themselves (gemm_dgrad), and the GEGLU pre-activation is recomputed by one GEMM."""
+        gradients read the forward weights themselves (gemm_dgrad), and the GEGLU pre-activation is recomputed by one GEMM.
+        params=False computes dx alone (a frozen block): no weight gradient and no GroupNorm affine gradient; grads is then
+        empty (the LayerNorm kernel still forms its affine gradients, which are dropped)."""
         P, G, p, heads = self.p, self.cfg.norm_groups, rec["p"], rec["heads"]
         b = p + ".transformer_blocks.0"
         x = rec["x"]
@@ -247,14 +254,17 @@ class _UNetCommon(_Base):
         grads = {}
 
         def lin(name, dy, xin, bias=True):
-            dw, db = D.gemm_wgrad(dy, xin, bias=bias)
-            grads[name + ".w"] = dw
-            if bias:
-                grads[name + ".bias"] = db
+            if params:
+                dw, db = D.gemm_wgrad(dy, xin, bias=bias)
+                grads[name + ".w"] = dw
+                if bias:
+                    grads[name + ".bias"] = db
             return D.gemm_dgrad(dy, P[name + ".w"])
 
         def ln(name, h, dn, dadd):
-            dh, grads[name + ".weight"], grads[name + ".bias"] = D.layernorm_bwd(h, dn, P[name + ".weight"], dx_add=dadd)
+            dh, dg, db = D.layernorm_bwd(h, dn, P[name + ".weight"], dx_add=dadd)
+            if params:
+                grads[name + ".weight"], grads[name + ".bias"] = dg, db
             return dh
 
         dy = dout.contiguous().view(M, C)
@@ -268,7 +278,8 @@ class _UNetCommon(_Base):
         d_kv = torch.empty_like(kv)
         dq2, _, _ = D.attention_bwd(rec["q"], kv[..., :C], kv[..., C:], rec["o2"], do2, rec["lse2"], heads,
                                     dk=d_kv[..., :C], dv=d_kv[..., C:])
-        grads[b + ".attn2.kv.w"], _ = D.gemm_wgrad(d_kv, rec["ctx"])
+        if params:
+            grads[b + ".attn2.kv.w"], _ = D.gemm_wgrad(d_kv, rec["ctx"])
         dn2 = lin(b + ".attn2.to_q", dq2, rec["n2"], bias=False)
         dh1 = ln(b + ".norm2", rec["h1"], dn2, dh2)
         do1 = lin(b + ".attn1.to_out.0", dh1, rec["o1"]).view(n, H * W, C)
@@ -281,7 +292,8 @@ class _UNetCommon(_Base):
         dhN = lin(p + ".proj_in", dh0, rec["hN"].view(M, C)).view(n, H, W, C)
         gm, bt = P[p + ".norm.weight"], P[p + ".norm.bias"]
         dx = D.groupnorm_bwd(x, dhN, gm, bt, rec["stats"], G, 1e-6, dx_add=dout.contiguous())
-        grads[p + ".norm.weight"], grads[p + ".norm.bias"] = D.groupnorm_affine_grad(x, dhN, gm, bt, rec["stats"], G)
+        if params:
+            grads[p + ".norm.weight"], grads[p + ".norm.bias"] = D.groupnorm_affine_grad(x, dhN, gm, bt, rec["stats"], G)
         return dx, grads
 
     def down_and_mid(self, sample, tproj, ctx, tape=None):
@@ -394,19 +406,38 @@ class UNet(_UNetCommon):
             if i < n - 1:
                 self._conv(f"up_blocks.{i}.upsamplers.0.conv")
         self._norm("conv_norm_out"); self._conv("conv_out")
+        # conv_out's weight with its 4 output rows zero-padded to 64, the Cout that conv2d_dgrad needs, for the decoder's
+        # input gradient (backward_residuals).  A copy made once is valid only because the UNet is frozen, both in the
+        # guidance loop and in ControlNet training; VAEEncoder's .wd copies rely on the same fact.
+        w_out = self.p["conv_out.w"]
+        self.conv_out_w64 = torch.zeros(64, w_out.shape[1], device=self.dev, dtype=self.dt)
+        self.conv_out_w64[:w_out.shape[0]] = w_out
         self._finish_tproj()
 
-    def forward(self, sample_nhwc, t_f32, ctx, down_res=None, mid_res=None, csd=None):
+    def forward(self, sample_nhwc, t_f32, ctx, down_res=None, mid_res=None, csd=None, tape=None):
         """sample [N,h,w,64] (4 real channels), ctx [N,77,D] -> eps [N,4,h,w] fp32 (values rounded to the
         storage dtype, as the reference's `.sample.to(input_dtype)`).
         csd = dict(noise, w1mac, coef, grad, dlat, norms[, eps_out]): conv_out runs with the CSD combination fused
-        into its epilogue (D.conv2d_csd) and nothing is returned."""
+        into its epilogue (D.conv2d_csd) and nothing is returned.
+        With a tape (a dict) it records what backward_residuals needs, the decoder only (nothing upstream of the residuals
+        is trainable); the output is the same bits either way.  A tape and csd exclude each other."""
+        if tape is not None and csd is not None:
+            raise ValueError("UNet.forward: a tape records eps for the training loss; the CSD epilogue returns none")
         cfg, P = self.cfg, self.p
         tproj = self.time_embed(t_f32)
         sample = D.conv2d(sample_nhwc, P["conv_in.w"], 3, bias=P["conv_in.bias"])
         res, sample = self.down_and_mid(sample, tproj, ctx)
         if mid_res is not None:
             sample = D.axpby(sample.view(-1, sample.shape[-1]), 1.0, mid_res.view(-1, sample.shape[-1]), 1.0).view(sample.shape)
+        up = tape.setdefault("up", []) if tape is not None else None
+
+        def rec(**kw):
+            if up is None:
+                return None
+            up.append(kw)
+            return kw
+        if tape is not None:
+            tape["n_res"] = len(res)
         n = len(cfg.block_out_channels)
         for i in range(n):
             for j in range(cfg.layers_per_block + 1):
@@ -420,13 +451,17 @@ class UNet(_UNetCommon):
                 # skip + ControlNet residual, fused into the concat copy
                 D.axpby(skip.view(-1, C2), 1.0, down_res[k].view(-1, C2) if down_res is not None else None, 1.0,
                         out=c2[:, C1:])
-                sample = self.resnet(f"up_blocks.{i}.resnets.{j}", cat, tproj)
+                sample = self.resnet(f"up_blocks.{i}.resnets.{j}", cat, tproj, tape=rec(kind="resnet", C1=C1, k=k))
                 if i > 0:
-                    sample = self.transformer(f"up_blocks.{i}.attentions.{j}", sample, ctx, cfg.heads[n - 1 - i])
+                    sample = self.transformer(f"up_blocks.{i}.attentions.{j}", sample, ctx, cfg.heads[n - 1 - i],
+                                              tape=rec(kind="transformer"))
             if i < n - 1:
                 pn = f"up_blocks.{i}.upsamplers.0.conv"
+                rec(kind="upsample", p=pn)
                 sample = D.conv2d(D.upsample2x(sample), P[pn + ".w"], 3, bias=P[pn + ".bias"])
-        h, _ = D.groupnorm(sample, P["conv_norm_out.weight"], P["conv_norm_out.bias"], cfg.norm_groups, 1e-5, silu=True)
+        h, st = D.groupnorm(sample, P["conv_norm_out.weight"], P["conv_norm_out.bias"], cfg.norm_groups, 1e-5, silu=True)
+        if tape is not None:
+            tape["norm_out"] = (sample, st)
         N_, H, W, _ = h.shape
         if csd is not None:
             D.conv2d_csd(h, P["conv_out.w"], P["conv_out.bias"], **csd)
@@ -434,6 +469,28 @@ class UNet(_UNetCommon):
         out = torch.empty(N_, H, W, 8, device=self.dev, dtype=self.dt)
         D.conv2d(h, P["conv_out.w"], 3, bias=P["conv_out.bias"], out=out[..., :cfg.out_channels])
         return D.nhwc_to_nchw_f32(out, cfg.out_channels)
+
+    def backward_residuals(self, tape, d_eps):
+        """Input gradient of the decoder of forward(..., down_res, mid_res, tape=tape) for d_eps [N, h, w, 64] NHWC (the
+        gradient of eps in its first 4 channels, zero padding; what mse_loss_grad writes): returns (d_down, d_mid), the
+        gradients of the twelve ControlNet down residuals and of the mid residual in their shapes and storage type, ready
+        for ControlNet.backward.  d_down[k] and d_mid are channel slices of an up resnet's input gradient: that resnet's
+        input is cat(sample, skip + down_res[k]).  No parameter gradient is formed (the UNet is frozen)."""
+        cfg, P = self.cfg, self.p
+        x, st = tape["norm_out"]
+        dh = D.conv2d_dgrad(d_eps, self.conv_out_w64, 3)
+        d = D.groupnorm_bwd(x, dh, P["conv_norm_out.weight"], P["conv_norm_out.bias"], st, cfg.norm_groups, 1e-5, silu=True)
+        d_down = [None] * tape["n_res"]
+        for r in reversed(tape["up"]):
+            if r["kind"] == "upsample":
+                d = D.upsample2x_bwd(D.conv2d_dgrad(d, P[r["p"] + ".w"], 3))
+            elif r["kind"] == "transformer":
+                d, _ = self.transformer_bwd(r, d, params=False)
+            else:
+                dx, _ = self.resnet_bwd(r, d, None, params=False)
+                d_down[r["k"]] = dx[..., r["C1"]:]
+                d = dx[..., :r["C1"]].contiguous()
+        return d_down, d
 
 
 class ControlNet(_UNetCommon):
@@ -549,6 +606,23 @@ class ControlNet(_UNetCommon):
         grads.update(self.cond_embed_bwd(tape["cond"], dc))
         grads.update(self.time_embed_bwd(tape["time"], d_tproj))
         return grads
+
+
+def controlnet_loss_and_grads(unet: UNet, controlnet: ControlNet, sample_nhwc, t, ctx, cond_nhwc, target,
+                              conditioning_scale=1.0, grad_scale=1.0):
+    """Loss and ControlNet gradients of one ControlNet training step (controlnet_train/diffusers_train_controlnet.py:
+    F.mse_loss(unet(noisy, t, ctx, down_res, mid_res).float(), target.float()), then accelerator.backward(loss)), the UNet
+    frozen.  sample_nhwc [N, h, w, 64] (the noisy latents, 4 real channels), cond_nhwc [Nc, 8h, 8w, 64], ctx [N, 77, D],
+    target fp32 NCHW [N, 4, h, w] (the noise, for epsilon prediction).  Returns (loss, grads): loss a 0-dim fp32 device
+    tensor, grads an fp32 tensor for every key of controlnet.p in its prepared layout, multiplied by grad_scale (a loss
+    scale for fp16 storage, 1 for bf16).  No host synchronisation, so the call can be captured in a CUDA graph."""
+    ctape, utape = {}, {}
+    down, mid = controlnet.forward(sample_nhwc, t, ctx, cond_nhwc, conditioning_scale, tape=ctape)
+    eps = unet.forward(sample_nhwc, t, ctx, down, mid, tape=utape)
+    loss, d_eps = D.mse_loss_grad(eps, target, unet.dt, grad_scale=grad_scale)
+    d_down, d_mid = unet.backward_residuals(utape, d_eps)
+    del utape           # the decoder's activations are not needed by the ControlNet backward
+    return loss, controlnet.backward(ctape, d_down, d_mid)
 
 
 # ================================================================================================ VAE encoder

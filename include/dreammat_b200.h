@@ -22,7 +22,8 @@
  * order (S and dP are recomputed rather than dQ added atomically); its delta scratch comes from the caller.  dm_groupnorm / dm_groupnorm_bwd (per-block partial sums), the bias gradient of
  * dm_conv2d_wgrad / dm_gemm_wgrad (per-block partial rows), dm_antialias_fwd / _bwd (per-pixel pair buckets) and
  * dm_hashgrid_mlp_bwd (int64 fixed-point grid gradient), dm_layernorm_bwd / dm_groupnorm_affine_grad (per-chunk partial
- * rows of the affine gradients) and dm_rowvec_grad (per-chunk partial rows, the same slot) need scratch for that which their signatures have no room for; the library allocates it once per device, on
+ * rows of the affine gradients), dm_rowvec_grad (per-chunk partial rows, the same slot) and dm_mse_loss_grad (per-block
+ * partial sums of the loss, added in block order, the same slot) need scratch for that which their signatures have no room for; the library allocates it once per device, on
  * the first call (not while the stream is being captured: run a call once before capturing it), and never frees it.  Calls
  * on one device must not run concurrently on two streams.
  */
@@ -381,6 +382,19 @@ int dm_silu_bwd(int bf16, const void* z, const void* dy, int64_t n, void* dx, vo
  * rows (library scratch, see DETERMINISM) are added in chunk order.  16-bit only (bf16 == 2: DM_EUNSUPPORTED). */
 int dm_rowvec_grad(int bf16, const void* dy, int64_t ld, int n_img, int rows_per_img, int N, void* out, int64_t ld_out,
                    void* stream);
+/* Adjoint of dm_upsample2x (nearest, zero_insert = 0): dy [n, 2H, 2W, C] -> dx [n, H, W, C], each element the sum of its
+ * 2x2 block, added in fp32 in a fixed order and rounded once.  C % 8 == 0, 16-byte aligned operands, positive extents,
+ * else DM_EINVAL before any launch; 16-bit only (bf16 == 2: DM_EUNSUPPORTED).  The backward of the UNet's Upsample2D. */
+int dm_upsample2x_bwd(int bf16, const void* dy, int n, int H, int W, int C, void* dx, void* stream);
+/* Loss and gradient of F.mse_loss(pred, target) (mean over all n*C*HW elements), the ControlNet training loss
+ * (controlnet_train/diffusers_train_controlnet.py: F.mse_loss(model_pred.float(), target.float())).  pred, target fp32 NCHW
+ * [n, C, HW] (pred as the UNet returns it); loss: one fp32 device scalar, unscaled; d_pred NHWC [n, HW, ld_d] in the storage
+ * type: grad_scale * 2 / (n*C*HW) * (pred - target), rounded once, for c < C and exactly 0 for C <= c < ld_d, so it feeds
+ * dm_conv2d_dgrad directly.  grad_scale is a loss scale (fp16 gradients underflow at 2 / numel; bf16 uses 1).
+ * ld_d % 64 == 0 and >= C, d_pred 16-byte aligned, pred / target / loss 4-byte aligned, else DM_EINVAL before any launch;
+ * 16-bit only (bf16 == 2: DM_EUNSUPPORTED).  No host synchronisation; deterministic (see DETERMINISM). */
+int dm_mse_loss_grad(int bf16, const float* pred, const float* target, int n, int C, int HW, float grad_scale, void* d_pred,
+                     int ld_d, float* loss, void* stream);
 
 /* Fused attention, head_dim 64: O = softmax(scale * Q K^T) V per (batch, head).  Q [batch,Nq,ldq],
  * K/V [batch,Nk,ldkv], O [batch,Nq,ldo]; head h occupies columns [64h, 64h+64) of every operand.
