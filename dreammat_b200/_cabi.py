@@ -114,6 +114,9 @@ SIGNATURES = {
     "dm_rowvec_grad": (C.c_int, [C.c_int, P, I64, C.c_int, C.c_int, C.c_int, P, I64, P]),
     "dm_upsample2x_bwd": (C.c_int, [C.c_int, P] + [C.c_int] * 4 + [P, P]),
     "dm_mse_loss_grad": (C.c_int, [C.c_int, P, P, C.c_int, C.c_int, C.c_int, F, P, C.c_int, P, P]),
+    "dm_grad_sumsq": (C.c_int, [P, I64, P, P]),
+    "dm_adamw_prepare": (C.c_int, [P, P, C.c_double, C.c_double, F, F, P]),
+    "dm_adamw_step": (C.c_int, [C.c_int, P, P, P, P, P, I64, P, C.c_double, C.c_double, F, F, P]),
 }
 
 

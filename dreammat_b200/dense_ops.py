@@ -215,10 +215,23 @@ def _wgrad_storage(t):
     return bf
 
 
-def conv2d_wgrad(x, dy, ksize, stride=1, pad=(1, 1), out_hw=None, bias=False):
+def _f32_out(t, shape, like):
+    """The fp32 output of a parameter-gradient kernel: a fresh tensor, or the caller's (a view of a flat gradient arena),
+    which the kernel then writes in place of allocating."""
+    if t is None:
+        return torch.empty(shape, device=like.device, dtype=torch.float32)
+    if (t.dtype != torch.float32 or tuple(t.shape) != tuple(shape) or not t.is_contiguous() or t.data_ptr() % 16
+            or t.device != like.device):
+        raise ValueError(f"gradient output must be a contiguous, 16-byte aligned fp32 tensor of shape {tuple(shape)} on "
+                         f"{like.device}; got {t.dtype} {tuple(t.shape)} strides {t.stride()} on {t.device}")
+    return t
+
+
+def conv2d_wgrad(x, dy, ksize, stride=1, pad=(1, 1), out_hw=None, bias=False, dw=None, db=None):
     """Weight (and bias) gradient of conv2d(x, w, ksize, stride, pad, out_hw) for the output gradient dy [n,Ho,Wo,Cout],
     which may be a channel slice of a wider buffer (its pixel stride is passed on).  Returns (dw, db): dw [Cout, k*k*Cin]
-    fp32 in conv2d's weight layout (tap-major, channel-minor, padded channels included), db [Cout] fp32 or None."""
+    fp32 in conv2d's weight layout (tap-major, channel-minor, padded channels included), db [Cout] fp32 or None.  dw= / db=
+    are written instead of fresh tensors when given."""
     _ensure_workspace()
     bf = _wgrad_storage(x)
     assert dy.dtype == x.dtype and x.is_contiguous()
@@ -228,17 +241,17 @@ def conv2d_wgrad(x, dy, ksize, stride=1, pad=(1, 1), out_hw=None, bias=False):
     ld = dy.stride(2)
     assert dy.stride(1) == Wo * ld and dy.stride(0) == Ho * Wo * ld
     Cout = dy.shape[3]
-    dw = torch.empty(Cout, ksize * ksize * Cin, device=x.device, dtype=torch.float32)
-    db = torch.empty(Cout, device=x.device, dtype=torch.float32) if bias else None
+    dw = _f32_out(dw, (Cout, ksize * ksize * Cin), x)
+    db = _f32_out(db, (Cout,), x) if bias else None
     check(lib().dm_conv2d_wgrad(bf, ptr_any(x), n, H, W, Cin, ptr_any(dy), ld, Cout, ksize, stride, pad[0], pad[1], Ho, Wo,
                                 ptr_any(dw), ptr_any(db) if bias else None, stream_ptr()), "dm_conv2d_wgrad")
     return dw, db
 
 
-def gemm_wgrad(dy, x, bias=False):
+def gemm_wgrad(dy, x, bias=False, dw=None, db=None):
     """Weight (and bias) gradient of gemm(x, w) = x w^T for the output gradient dy: dy [.., M, N], x [.., M, K] (leading
     dims fold into M; row strides allowed, e.g. a column slice of a fused projection).  Returns (dw, db): dw [N, K] fp32 in
-    the layout and row order of w, db [N] fp32 or None."""
+    the layout and row order of w, db [N] fp32 or None.  dw= / db= are written instead of fresh tensors when given."""
     _ensure_workspace()
     bf = _wgrad_storage(x)
     assert dy.dtype == x.dtype and dy.stride(-1) == 1 and x.stride(-1) == 1
@@ -246,8 +259,8 @@ def gemm_wgrad(dy, x, bias=False):
     M, N = dy2.shape
     K = x2.shape[1]
     assert x2.shape[0] == M
-    dw = torch.empty(N, K, device=x.device, dtype=torch.float32)
-    db = torch.empty(N, device=x.device, dtype=torch.float32) if bias else None
+    dw = _f32_out(dw, (N, K), x)
+    db = _f32_out(db, (N,), x) if bias else None
     check(lib().dm_gemm_wgrad(bf, ptr_any(dy2), dy2.stride(0), ptr_any(x2), x2.stride(0), M, N, K, ptr_any(dw),
                               ptr_any(db) if bias else None, stream_ptr()), "dm_gemm_wgrad")
     return dw, db
@@ -384,30 +397,28 @@ def layernorm(x, gamma, beta, eps=1e-5):
     return y
 
 
-def layernorm_bwd(x, dy, gamma, eps=1e-5, dx_add=None):
-    """Backward of layernorm(x, gamma, beta, eps): returns (dx [storage dtype] (+ dx_add), dgamma, dbeta [C] fp32).
-    16-bit storage only; deterministic."""
+def layernorm_bwd(x, dy, gamma, eps=1e-5, dx_add=None, dgamma=None, dbeta=None):
+    """Backward of layernorm(x, gamma, beta, eps): returns (dx [storage dtype] (+ dx_add), dgamma, dbeta [C] fp32), the
+    last two written into dgamma= / dbeta= when given.  16-bit storage only; deterministic."""
     bf = _is_bf16(x)
     assert x.is_contiguous() and dy.is_contiguous() and dy.shape == x.shape
     assert dx_add is None or (dx_add.is_contiguous() and dx_add.shape == x.shape)
     Cc = x.shape[-1]
     dx = torch.empty_like(x)
-    dg = torch.empty(Cc, device=x.device, dtype=torch.float32)
-    db = torch.empty(Cc, device=x.device, dtype=torch.float32)
+    dg, db = _f32_out(dgamma, (Cc,), x), _f32_out(dbeta, (Cc,), x)
     check(lib().dm_layernorm_bwd(bf, ptr_any(x), ptr_any(dy), x.numel() // Cc, Cc, ptr_any(gamma), eps,
                                  ptr_any(dx_add) if dx_add is not None else None, ptr_any(dx), ptr_any(dg), ptr_any(db),
                                  stream_ptr()), "dm_layernorm_bwd")
     return dx, dg, db
 
 
-def groupnorm_affine_grad(x, dz, gamma, beta, stats, groups=32, silu=False):
+def groupnorm_affine_grad(x, dz, gamma, beta, stats, groups=32, silu=False, dgamma=None, dbeta=None):
     """(dgamma, dbeta) [C] fp32 of groupnorm(x, gamma, beta, groups, silu=silu) for the output gradient dz (x, dz dense
-    [n, H, W, C]; stats from groupnorm).  16-bit storage only; deterministic."""
+    [n, H, W, C]; stats from groupnorm), written into dgamma= / dbeta= when given.  16-bit storage only; deterministic."""
     bf = _is_bf16(x)
     n, Hh, W, Cc = x.shape
     assert x.is_contiguous() and dz.is_contiguous() and dz.shape == x.shape
-    dg = torch.empty(Cc, device=x.device, dtype=torch.float32)
-    db = torch.empty(Cc, device=x.device, dtype=torch.float32)
+    dg, db = _f32_out(dgamma, (Cc,), x), _f32_out(dbeta, (Cc,), x)
     check(lib().dm_groupnorm_affine_grad(bf, ptr_any(x), ptr_any(dz), n, Hh * W, Cc, groups, ptr_any(gamma), ptr_any(beta),
                                          1 if silu else 0, ptr_any(stats), ptr_any(dg), ptr_any(db), stream_ptr()),
           "dm_groupnorm_affine_grad")
@@ -480,6 +491,46 @@ def mse_loss_grad(pred, target, dtype, ld=64, grad_scale=1.0):
     check(lib().dm_mse_loss_grad(_dt_code(dtype), ptr_any(pred), ptr_any(target), n, Cc, H * W, grad_scale, ptr_any(d_pred), ld,
                                  ptr_any(loss), stream_ptr()), "dm_mse_loss_grad")
     return loss, d_pred
+
+
+def grad_sumsq(g, out=None):
+    """Squared L2 norm of a flat fp32 gradient buffer -> 0-dim fp32 device tensor (or into `out`).  Deterministic."""
+    assert g.dtype == torch.float32 and g.dim() == 1 and g.is_contiguous()
+    if out is None:
+        out = torch.empty((), device=g.device, dtype=torch.float32)
+    check(lib().dm_grad_sumsq(ptr_any(g), g.numel(), ptr_any(out), stream_ptr()), "dm_grad_sumsq")
+    return out
+
+
+ADAMW_STATE_WORDS = 8     # dm_adamw_state: lr, step, skipped_steps, skip, grad_norm, gmul, step_size, inv_sqrt_bc2
+
+
+def adamw_state(lr, device):
+    """A zeroed device-resident dm_adamw_state holding lr: an fp32 tensor of 8 words whose words 1..3 are int32 (view them
+    with .view(torch.int32))."""
+    st = torch.zeros(ADAMW_STATE_WORDS, device=device, dtype=torch.float32)
+    st[0] = lr
+    return st
+
+
+def adamw_prepare(sumsq, state, betas, max_grad_norm, inv_grad_scale):
+    """Clip factor, bias corrections and the skip flag of this step into `state` (dm_adamw_prepare); max_grad_norm None
+    disables clipping."""
+    assert state.dtype == torch.float32 and state.numel() == ADAMW_STATE_WORDS and sumsq.dtype == torch.float32
+    check(lib().dm_adamw_prepare(ptr_any(sumsq), ptr_any(state), betas[0], betas[1],
+                                 float("inf") if max_grad_norm is None else max_grad_norm, inv_grad_scale, stream_ptr()),
+          "dm_adamw_prepare")
+
+
+def adamw_step(master, m, v, g, w16, state, betas, eps, weight_decay):
+    """torch.optim.AdamW.step over flat fp32 master / m / v with the flat fp32 gradient g, the updated weights also rounded
+    into the flat 16-bit copy w16 (dm_adamw_step).  The scalars of the step come from `state` (adamw_prepare)."""
+    n = master.numel()
+    for t in (master, m, v, g):
+        assert t.dtype == torch.float32 and t.dim() == 1 and t.numel() == n and t.is_contiguous()
+    assert w16.dim() == 1 and w16.numel() == n and w16.is_contiguous()
+    check(lib().dm_adamw_step(_is_bf16(w16), ptr_any(master), ptr_any(m), ptr_any(v), ptr_any(g), ptr_any(w16), n,
+                              ptr_any(state), betas[0], betas[1], eps, weight_decay, stream_ptr()), "dm_adamw_step")
 
 
 def axpby(s1, a=1.0, s2=None, b=1.0, out=None):

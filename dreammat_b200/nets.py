@@ -23,6 +23,12 @@ def _r64(c):
     return (c + 63) // 64 * 64
 
 
+def _dst(into, **keys):
+    """keyword arguments that make a dense_ops gradient call write into[key] (into: parameter name -> preallocated fp32
+    tensor, e.g. the views of a flat gradient arena); none without `into`, and the call allocates as usual"""
+    return {} if into is None else {arg: into[k] for arg, k in keys.items()}
+
+
 class _Base:
     def __init__(self, w: Dict[str, torch.Tensor], device, dtype):
         self.dev, self.dt = device, dtype
@@ -139,17 +145,17 @@ class _UNetCommon(_Base):
             tape.update(e0=e0, e1=e1, e2=e2)
         return D.gemm(e2, P["tproj.w"], bias=P["tproj.b"])   # [N, sum Cout]
 
-    def time_embed_bwd(self, rec, d_tproj):
+    def time_embed_bwd(self, rec, d_tproj, into=None):
         """Backward of time_embed(t, tape=rec) for d_tproj [N, sum Cout] (every resnet_bwd has written its columns):
         gradients of tproj and both time_embedding linears.  The fused-SiLU GEMMs kept only their activated outputs, so
-        each pre-activation is recomputed by the same GEMM without the activation (M is the batch)."""
+        each pre-activation is recomputed by the same GEMM without the activation (M is the batch).  `into`: see backward."""
         P, grads = self.p, {}
-        grads["tproj.w"], grads["tproj.b"] = D.gemm_wgrad(d_tproj, rec["e2"], bias=True)
+        grads["tproj.w"], grads["tproj.b"] = D.gemm_wgrad(d_tproj, rec["e2"], bias=True, **_dst(into, dw="tproj.w", db="tproj.b"))
         d = D.gemm_dgrad(d_tproj, P["tproj.w"])
         for name, xin in (("time_embedding.linear_2", rec["e1"]), ("time_embedding.linear_1", rec["e0"])):
             z = D.gemm(xin, P[name + ".w"], bias=P[name + ".bias"])
             dz = D.silu_bwd(z, d)
-            grads[name + ".w"], grads[name + ".bias"] = D.gemm_wgrad(dz, xin, bias=True)
+            grads[name + ".w"], grads[name + ".bias"] = D.gemm_wgrad(dz, xin, bias=True, **_dst(into, dw=name + ".w", db=name + ".bias"))
             if xin is not rec["e0"]:
                 d = D.gemm_dgrad(dz, P[name + ".w"])
         return grads
@@ -172,12 +178,12 @@ class _UNetCommon(_Base):
             tape.update(p=p, x=xs, st1=st1, h1=h1, st2=st2)
         return D.conv2d(h, P[p + ".conv2.w"], 3, bias=P[p + ".conv2.bias"], residual=sc, out=out)
 
-    def resnet_bwd(self, rec, dout, d_tproj, dx_add=None, params=True):
+    def resnet_bwd(self, rec, dout, d_tproj, dx_add=None, params=True, into=None):
         """Backward of resnet(p, x, tproj, tape=rec) for the output gradient dout [n, H, W, Cout]: returns (dx, grads) and
         writes this resnet's columns of d_tproj [n, sum Cout].  dx_add is a second gradient of x (x also fed a skip
         output): it rides on the shortcut's input-gradient GEMM as its residual, or costs one add when the shortcut is the
         identity.  params=False computes dx alone (a frozen block): no parameter or d_tproj gradient (d_tproj may be None),
-        and none of the GroupNorm recomputations that only feed them; grads is then empty."""
+        and none of the GroupNorm recomputations that only feed them; grads is then empty.  `into`: see ControlNet.backward."""
         P, G, p, x, h1 = self.p, self.cfg.norm_groups, rec["p"], rec["x"], rec["h1"]
         n, H, W, Cin = x.shape
         off, co = self.tproj_off[p]
@@ -186,18 +192,20 @@ class _UNetCommon(_Base):
         dout = dout if dout.is_contiguous() else dout.contiguous()
         if params:
             a2, _ = D.groupnorm(h1, g2, b2, G, 1e-5, silu=True)                  # conv2's input, recomputed
-            grads[p + ".conv2.w"], grads[p + ".conv2.bias"] = D.conv2d_wgrad(a2, dout, 3, bias=True)
+            grads[p + ".conv2.w"], grads[p + ".conv2.bias"] = D.conv2d_wgrad(a2, dout, 3, bias=True, **_dst(into, dw=p + ".conv2.w", db=p + ".conv2.bias"))
         da2 = D.conv2d_dgrad(dout, P[p + ".conv2.w"], 3)
         dh1 = D.groupnorm_bwd(h1, da2, g2, b2, rec["st2"], G, 1e-5, silu=True)
         if params:
-            grads[p + ".norm2.weight"], grads[p + ".norm2.bias"] = D.groupnorm_affine_grad(h1, da2, g2, b2, rec["st2"], G, silu=True)
+            grads[p + ".norm2.weight"], grads[p + ".norm2.bias"] = D.groupnorm_affine_grad(
+                h1, da2, g2, b2, rec["st2"], G, silu=True, **_dst(into, dgamma=p + ".norm2.weight", dbeta=p + ".norm2.bias"))
             D.rowvec_grad(dh1, n, out=d_tproj[:, off:off + co])
             a1, _ = D.groupnorm(x, g1, b1, G, 1e-5, silu=True)                   # conv1's input, recomputed
-            grads[p + ".conv1.w"], grads[p + ".conv1.bias"] = D.conv2d_wgrad(a1, dh1, 3, bias=True)
+            grads[p + ".conv1.w"], grads[p + ".conv1.bias"] = D.conv2d_wgrad(a1, dh1, 3, bias=True, **_dst(into, dw=p + ".conv1.w", db=p + ".conv1.bias"))
         da1 = D.conv2d_dgrad(dh1, P[p + ".conv1.w"], 3)
         if p + ".conv_shortcut.w" in P:
             if params:
-                grads[p + ".conv_shortcut.w"], grads[p + ".conv_shortcut.bias"] = D.gemm_wgrad(dout.view(-1, co), x.view(-1, Cin), bias=True)
+                grads[p + ".conv_shortcut.w"], grads[p + ".conv_shortcut.bias"] = D.gemm_wgrad(
+                    dout.view(-1, co), x.view(-1, Cin), bias=True, **_dst(into, dw=p + ".conv_shortcut.w", db=p + ".conv_shortcut.bias"))
             dsc = D.gemm_dgrad(dout.view(-1, co), P[p + ".conv_shortcut.w"],
                                residual=dx_add.view(-1, Cin) if dx_add is not None else None).view(n, H, W, Cin)
         elif dx_add is not None:
@@ -206,7 +214,8 @@ class _UNetCommon(_Base):
             dsc = dout
         dx = D.groupnorm_bwd(x, da1, g1, b1, rec["st1"], G, 1e-5, silu=True, dx_add=dsc)
         if params:
-            grads[p + ".norm1.weight"], grads[p + ".norm1.bias"] = D.groupnorm_affine_grad(x, da1, g1, b1, rec["st1"], G, silu=True)
+            grads[p + ".norm1.weight"], grads[p + ".norm1.bias"] = D.groupnorm_affine_grad(
+                x, da1, g1, b1, rec["st1"], G, silu=True, **_dst(into, dgamma=p + ".norm1.weight", dbeta=p + ".norm1.bias"))
         return dx, grads
 
     def transformer(self, p, x, ctx, heads, tape=None):
@@ -239,13 +248,13 @@ class _UNetCommon(_Base):
                         n2=n2, q=q, kv=kv, o2=o2, lse2=lse2, h2=h2, n3=n3, f=f, h3=h3)
         return D.gemm(h3, P[p + ".proj_out.w"], bias=P[p + ".proj_out.bias"], residual=xs.view(M, C)).view(n, H, W, C)
 
-    def transformer_bwd(self, rec, dout, params=True):
+    def transformer_bwd(self, rec, dout, params=True, into=None):
         """Backward of transformer(p, x, ctx, heads, tape=rec) for the output gradient dout [n, H, W, C]: returns (dx,
         grads), grads mapping each prepared parameter name of the block to its fp32 gradient in the prepared layout (qkv /
         kv fused, ff.net.0.proj value / gate interleaved).  ctx gets no gradient (the text encoder is frozen).  The input
         gradients read the forward weights themselves (gemm_dgrad), and the GEGLU pre-activation is recomputed by one GEMM.
         params=False computes dx alone (a frozen block): no weight gradient and no GroupNorm affine gradient; grads is then
-        empty (the LayerNorm kernel still forms its affine gradients, which are dropped)."""
+        empty (the LayerNorm kernel still forms its affine gradients, which are dropped).  `into`: see ControlNet.backward."""
         P, G, p, heads = self.p, self.cfg.norm_groups, rec["p"], rec["heads"]
         b = p + ".transformer_blocks.0"
         x = rec["x"]
@@ -255,14 +264,16 @@ class _UNetCommon(_Base):
 
         def lin(name, dy, xin, bias=True):
             if params:
-                dw, db = D.gemm_wgrad(dy, xin, bias=bias)
+                dw, db = D.gemm_wgrad(dy, xin, bias=bias, **(_dst(into, dw=name + ".w", db=name + ".bias") if bias else
+                                                            _dst(into, dw=name + ".w")))
                 grads[name + ".w"] = dw
                 if bias:
                     grads[name + ".bias"] = db
             return D.gemm_dgrad(dy, P[name + ".w"])
 
         def ln(name, h, dn, dadd):
-            dh, dg, db = D.layernorm_bwd(h, dn, P[name + ".weight"], dx_add=dadd)
+            dh, dg, db = D.layernorm_bwd(h, dn, P[name + ".weight"], dx_add=dadd,
+                                         **(_dst(into, dgamma=name + ".weight", dbeta=name + ".bias") if params else {}))
             if params:
                 grads[name + ".weight"], grads[name + ".bias"] = dg, db
             return dh
@@ -279,7 +290,7 @@ class _UNetCommon(_Base):
         dq2, _, _ = D.attention_bwd(rec["q"], kv[..., :C], kv[..., C:], rec["o2"], do2, rec["lse2"], heads,
                                     dk=d_kv[..., :C], dv=d_kv[..., C:])
         if params:
-            grads[b + ".attn2.kv.w"], _ = D.gemm_wgrad(d_kv, rec["ctx"])
+            grads[b + ".attn2.kv.w"], _ = D.gemm_wgrad(d_kv, rec["ctx"], **_dst(into, dw=b + ".attn2.kv.w"))
         dn2 = lin(b + ".attn2.to_q", dq2, rec["n2"], bias=False)
         dh1 = ln(b + ".norm2", rec["h1"], dn2, dh2)
         do1 = lin(b + ".attn1.to_out.0", dh1, rec["o1"]).view(n, H * W, C)
@@ -293,7 +304,8 @@ class _UNetCommon(_Base):
         gm, bt = P[p + ".norm.weight"], P[p + ".norm.bias"]
         dx = D.groupnorm_bwd(x, dhN, gm, bt, rec["stats"], G, 1e-6, dx_add=dout.contiguous())
         if params:
-            grads[p + ".norm.weight"], grads[p + ".norm.bias"] = D.groupnorm_affine_grad(x, dhN, gm, bt, rec["stats"], G)
+            grads[p + ".norm.weight"], grads[p + ".norm.bias"] = D.groupnorm_affine_grad(
+                x, dhN, gm, bt, rec["stats"], G, **_dst(into, dgamma=p + ".norm.weight", dbeta=p + ".norm.bias"))
         return dx, grads
 
     def down_and_mid(self, sample, tproj, ctx, tape=None):
@@ -333,26 +345,27 @@ class _UNetCommon(_Base):
         sample = self.resnet("mid_block.resnets.1", sample, tproj, tape=rec("resnet"))
         return res, sample
 
-    def down_and_mid_bwd(self, tape, d_res, d_mid, d_tproj):
+    def down_and_mid_bwd(self, tape, d_res, d_mid, d_tproj, into=None):
         """Backward of down_and_mid(sample, tproj, ctx, tape=tape): d_res[k] is the gradient of skip output res[k] (None
         for none), d_mid that of the mid block's output.  Walks the tape in reverse; returns (d_sample, grads) with d_res[0]
         included in d_sample, and fills d_tproj.  Where an activation feeds a skip output and the next layer, the skip's
         gradient is the residual of that layer's input-gradient kernel (downsampler, resnet with a shortcut) or one add
-        (resnet whose shortcut is the identity)."""
+        (resnet whose shortcut is the identity).  `into`: see ControlNet.backward."""
         grads = {}
         d = d_mid
         for r in reversed(tape):
             extra = d_res[r["skip_in"]] if r["skip_in"] is not None else None
             if r["kind"] == "resnet":
-                d, g = self.resnet_bwd(r, d, d_tproj, dx_add=extra)
+                d, g = self.resnet_bwd(r, d, d_tproj, dx_add=extra, into=into)
             elif r["kind"] == "transformer":
                 assert extra is None      # a transformer's input is a resnet's output, never a skip output
-                d, g = self.transformer_bwd(r, d)
+                d, g = self.transformer_bwd(r, d, into=into)
             else:
                 pn = r["p"]
                 d = d if d.is_contiguous() else d.contiguous()
                 g = {}
-                g[pn + ".w"], g[pn + ".bias"] = D.conv2d_wgrad(r["x"], d, 3, stride=2, pad=(1, 1), bias=True)
+                g[pn + ".w"], g[pn + ".bias"] = D.conv2d_wgrad(r["x"], d, 3, stride=2, pad=(1, 1), bias=True,
+                                                                **_dst(into, dw=pn + ".w", db=pn + ".bias"))
                 d = D.conv2d_dgrad(D.upsample2x(d, zero_insert=True), self.p[pn + ".w"], 3, pad=(1, 1), residual=extra)
             grads.update(g)
         return d, grads
@@ -531,19 +544,20 @@ class ControlNet(_UNetCommon):
             c = D.conv2d(c, P[pn + ".w"], 3, stride=stride, pad=(1, 1), bias=P[pn + ".bias"], act=act)
         return c
 
-    def cond_embed_bwd(self, tape, dc):
+    def cond_embed_bwd(self, tape, dc, into=None):
         """Backward of cond_embed(cond, tape=tape) for the embedding's gradient dc: gradients of its eight convolutions (the
         condition itself gets none).  The forward fuses SiLU into the convolution and keeps only the activated output, so
         each pre-activation is recomputed by the same convolution without the activation.  Padded channels (22 -> 64
         condition, 16 / 32 / 96 -> 64 / 64 / 128 widths) carry zero activations and zero weights, so their gradients come
-        out exactly zero."""
+        out exactly zero.  `into`: see backward."""
         P, grads = self.p, {}
         d = dc if dc.is_contiguous() else dc.contiguous()
         for k, (pn, stride, act, x) in reversed(list(enumerate(tape))):
             if act is not None:
                 z = D.conv2d(x, P[pn + ".w"], 3, stride=stride, pad=(1, 1), bias=P[pn + ".bias"])
                 d = D.silu_bwd(z, d)
-            grads[pn + ".w"], grads[pn + ".bias"] = D.conv2d_wgrad(x, d, 3, stride=stride, pad=(1, 1), bias=True)
+            grads[pn + ".w"], grads[pn + ".bias"] = D.conv2d_wgrad(x, d, 3, stride=stride, pad=(1, 1), bias=True,
+                                                                  **_dst(into, dw=pn + ".w", db=pn + ".bias"))
             if k > 0:
                 d = D.conv2d_dgrad(D.upsample2x(d, zero_insert=True) if stride == 2 else d, P[pn + ".w"], 3, pad=(1, 1))
         return grads
@@ -577,11 +591,14 @@ class ControlNet(_UNetCommon):
                      out_scale=conditioning_scale).view(n, H, W, C)
         return down, mid
 
-    def backward(self, tape, d_down, d_mid):
+    def backward(self, tape, d_down, d_mid, into=None):
         """Gradients of every parameter from the gradients of forward(..., tape=tape)'s fourteen outputs: d_down[i] / d_mid
         in the outputs' shapes and storage type.  Returns grads mapping EVERY key of self.p to an fp32 tensor in that key's
         prepared layout (grads_to_state_dict maps them to diffusers names).  The noisy latents, the condition, the
-        timesteps and ctx get no gradient."""
+        timesteps and ctx get no gradient.
+        into: a dict with a preallocated contiguous fp32 tensor of p[key]'s shape for every key of self.p (the views of a
+        flat gradient arena).  Every gradient kernel then writes its output there: nothing is allocated for a parameter
+        gradient, nothing is copied afterwards, and the returned dict is `into` itself."""
         P, scale = self.p, tape["scale"]
         grads = {}
 
@@ -590,39 +607,45 @@ class ControlNet(_UNetCommon):
             dy = dy.reshape(-1, C) if dy.is_contiguous() else dy.contiguous().view(-1, C)
             if scale != 1.0:      # out = scale * (W r + b): fold the scale into the gradient once
                 dy = D.axpby(dy, scale)
-            grads[name + ".w"], grads[name + ".bias"] = D.gemm_wgrad(dy, r.view(-1, C), bias=True)
+            grads[name + ".w"], grads[name + ".bias"] = D.gemm_wgrad(dy, r.view(-1, C), bias=True,
+                                                                     **_dst(into, dw=name + ".w", db=name + ".bias"))
             return D.gemm_dgrad(dy, P[name + ".w"]).view(r.shape)
 
         d_res = [zero_conv(f"controlnet_down_blocks.{i}", d_down[i], r) for i, r in enumerate(tape["res"])]
         d_m = zero_conv("controlnet_mid_block", d_mid, tape["mid"])
         d_tproj = torch.empty(tape["tproj_shape"], device=self.dev, dtype=self.dt)
-        d_sample, g = self.down_and_mid_bwd(tape["walk"], d_res, d_m, d_tproj)
+        d_sample, g = self.down_and_mid_bwd(tape["walk"], d_res, d_m, d_tproj, into=into)
         grads.update(g)
-        grads["conv_in.w"], grads["conv_in.bias"] = D.conv2d_wgrad(tape["sample_in"], d_sample, 3, bias=True)
+        grads["conv_in.w"], grads["conv_in.bias"] = D.conv2d_wgrad(tape["sample_in"], d_sample, 3, bias=True,
+                                                                    **_dst(into, dw="conv_in.w", db="conv_in.bias"))
         B = tape["n_cond"]
         dc = d_sample[:B]             # the embedding is shared by the rep copies of a view: its gradient is their sum
         for k in range(1, d_sample.shape[0] // B):
             dc = D.axpby(dc.reshape(-1, dc.shape[-1]), 1.0, d_sample[k * B:(k + 1) * B].view(-1, dc.shape[-1]), 1.0).view(dc.shape)
-        grads.update(self.cond_embed_bwd(tape["cond"], dc))
-        grads.update(self.time_embed_bwd(tape["time"], d_tproj))
-        return grads
+        grads.update(self.cond_embed_bwd(tape["cond"], dc, into=into))
+        grads.update(self.time_embed_bwd(tape["time"], d_tproj, into=into))
+        if into is None:
+            return grads
+        assert grads.keys() == into.keys() and all(grads[k] is into[k] for k in grads)
+        return into
 
 
 def controlnet_loss_and_grads(unet: UNet, controlnet: ControlNet, sample_nhwc, t, ctx, cond_nhwc, target,
-                              conditioning_scale=1.0, grad_scale=1.0):
+                              conditioning_scale=1.0, grad_scale=1.0, into=None):
     """Loss and ControlNet gradients of one ControlNet training step (controlnet_train/diffusers_train_controlnet.py:
     F.mse_loss(unet(noisy, t, ctx, down_res, mid_res).float(), target.float()), then accelerator.backward(loss)), the UNet
     frozen.  sample_nhwc [N, h, w, 64] (the noisy latents, 4 real channels), cond_nhwc [Nc, 8h, 8w, 64], ctx [N, 77, D],
     target fp32 NCHW [N, 4, h, w] (the noise, for epsilon prediction).  Returns (loss, grads): loss a 0-dim fp32 device
     tensor, grads an fp32 tensor for every key of controlnet.p in its prepared layout, multiplied by grad_scale (a loss
-    scale for fp16 storage, 1 for bf16).  No host synchronisation, so the call can be captured in a CUDA graph."""
+    scale for fp16 storage, 1 for bf16).  With `into` (ControlNet.backward) the gradients are written there and grads is
+    `into`.  No host synchronisation, so the call can be captured in a CUDA graph."""
     ctape, utape = {}, {}
     down, mid = controlnet.forward(sample_nhwc, t, ctx, cond_nhwc, conditioning_scale, tape=ctape)
     eps = unet.forward(sample_nhwc, t, ctx, down, mid, tape=utape)
     loss, d_eps = D.mse_loss_grad(eps, target, unet.dt, grad_scale=grad_scale)
     d_down, d_mid = unet.backward_residuals(utape, d_eps)
     del utape           # the decoder's activations are not needed by the ControlNet backward
-    return loss, controlnet.backward(ctape, d_down, d_mid)
+    return loss, controlnet.backward(ctape, d_down, d_mid, into=into)
 
 
 # ================================================================================================ VAE encoder

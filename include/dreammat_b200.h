@@ -23,7 +23,8 @@
  * dm_conv2d_wgrad / dm_gemm_wgrad (per-block partial rows), dm_antialias_fwd / _bwd (per-pixel pair buckets) and
  * dm_hashgrid_mlp_bwd (int64 fixed-point grid gradient), dm_layernorm_bwd / dm_groupnorm_affine_grad (per-chunk partial
  * rows of the affine gradients), dm_rowvec_grad (per-chunk partial rows, the same slot) and dm_mse_loss_grad (per-block
- * partial sums of the loss, added in block order, the same slot) need scratch for that which their signatures have no room for; the library allocates it once per device, on
+ * partial sums of the loss, added in block order, the same slot) and dm_grad_sumsq (per-block partial sums of the squared
+ * gradient norm, added in block order, the same slot: at most 1056 floats) need scratch for that which their signatures have no room for; the library allocates it once per device, on
  * the first call (not while the stream is being captured: run a call once before capturing it), and never frees it.  Calls
  * on one device must not run concurrently on two streams.
  */
@@ -395,6 +396,41 @@ int dm_upsample2x_bwd(int bf16, const void* dy, int n, int H, int W, int C, void
  * 16-bit only (bf16 == 2: DM_EUNSUPPORTED).  No host synchronisation; deterministic (see DETERMINISM). */
 int dm_mse_loss_grad(int bf16, const float* pred, const float* target, int n, int C, int HW, float grad_scale, void* d_pred,
                      int ld_d, float* loss, void* stream);
+
+/* ------------------------------------------------------------------ optimizer of the ControlNet training step
+ * controlnet_train/diffusers_train_controlnet.py: accelerator.clip_grad_norm_(controlnet.parameters(), max_grad_norm);
+ * optimizer.step() with torch.optim.AdamW, on fp32 master weights with a 16-bit copy for the forward / backward kernels.
+ * All parameters live in flat arenas with one element order; whatever changes from step to step is read from this
+ * device-resident struct, so a captured CUDA graph of the step keeps working while the host changes lr. */
+typedef struct {
+    float lr;               /* in: written by the host (a small H2D copy between steps) */
+    int32_t step;           /* in/out: steps applied so far (t of the bias corrections after the increment) */
+    int32_t skipped_steps;  /* in/out: steps dropped because the gradient norm was not finite */
+    int32_t skip;           /* out of dm_adamw_prepare: 1 = dm_adamw_step writes nothing */
+    float grad_norm;        /* out: L2 norm of the unscaled gradient, before clipping (what clip_grad_norm_ returns) */
+    float gmul;             /* out: inv_grad_scale * min(1, max_grad_norm / (grad_norm + 1e-6)) */
+    float step_size;        /* out: lr / (1 - beta1^step) */
+    float inv_sqrt_bc2;     /* out: 1 / sqrt(1 - beta2^step) */
+} dm_adamw_state;
+/* *sumsq = sum of g[i]^2 over the flat fp32 buffer g[n] (any n >= 1; g 16-byte aligned), else DM_EINVAL before any launch.
+ * Deterministic: the grid depends on n alone, per-block sums are added in block order (library scratch, see DETERMINISM:
+ * run one call before capturing a graph).  No host synchronisation. */
+int dm_grad_sumsq(const float* g, int64_t n, float* sumsq, void* stream);
+/* One thread: fills the out fields of *state for this step from *sumsq (of the gradient multiplied by 1 / inv_grad_scale =
+ * loss scale x world size) and state->lr / step.  A non-finite norm sets skip and counts it (torch's GradScaler drops such a
+ * step); otherwise step is incremented.  The betas are doubles (as torch's are) and the two powers are taken in double.  beta1, beta2 in [0, 1), max_grad_norm >= 0
+ * (INFINITY: no clipping), inv_grad_scale positive and finite, else DM_EINVAL before any launch. */
+int dm_adamw_prepare(const float* sumsq, dm_adamw_state* state, double beta1, double beta2, float max_grad_norm,
+                     float inv_grad_scale, void* stream);
+/* torch.optim.AdamW.step (decoupled weight decay, no amsgrad) over the flat fp32 arenas master / m / v [n] with the
+ * gradient g [n] multiplied by state->gmul: master *= 1 - lr * weight_decay; m = lerp(m, g, 1 - beta1); v = beta2 v +
+ * (1 - beta2) g^2; master -= step_size * m / (sqrt(v) * inv_sqrt_bc2 + eps); w16[i] = master[i] rounded once to the
+ * storage type (bf16: 0 fp16, 1 bf16), the copy the forward and input-gradient kernels read.  With state->skip set nothing
+ * is written.  An element with zero weight, gradient and moments (channel padding) stays exactly zero.  Any n >= 1; the
+ * five arenas 16-byte aligned; betas in [0, 1); eps, weight_decay >= 0; else DM_EINVAL before any launch.  34 bytes of
+ * traffic per parameter with dm_grad_sumsq.  Deterministic; no host synchronisation. */
+int dm_adamw_step(int bf16, float* master, float* m, float* v, const float* g, void* w16, int64_t n,
+                  const dm_adamw_state* state, double beta1, double beta2, float eps, float weight_decay, void* stream);
 
 /* Fused attention, head_dim 64: O = softmax(scale * Q K^T) V per (batch, head).  Q [batch,Nq,ldq],
  * K/V [batch,Nk,ldkv], O [batch,Nq,ldo]; head h occupies columns [64h, 64h+64) of every operand.
